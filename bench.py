@@ -12,8 +12,13 @@ backward + optimizer update of one global batch through `easydist_compile`'s com
 Printed keys (one JSON line from rank 0): see the bench contract in the task statement;
 `value` = samples/s with inputs resident in HBM, `e2e` = the same through the public API with
 pinned-host inputs copied H2D and the loss read back D2H every step, `roofline` = the dominant
-kernel (tcgen05 GEMM) against the measured bf16 peak, `cpu_baseline` = the oracle port on the
-host cores (bounded sample).
+kernel (wgmma GEMM) against the bf16 peak, `cpu_baseline` = the oracle port on the host cores
+(bounded sample).
+
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step handed back to its
+caller: the loss, and a fixed seeded sample of every parameter and momentum buffer it updated
+(`DIR/<name>.npy`, float32).  The inputs are seeded, so two builds run with the same arguments
+can be compared output for output.
 """
 import argparse
 import json
@@ -55,7 +60,15 @@ def parse_args():
                          "allocates fresh operands for every launch)")
     ap.add_argument("--no-parity", action="store_true",
                     help="skip the pre-timing parity leg (compiled N-GPU steps vs vanilla fp32)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (loss, sampled parameters and momentum "
+                         "buffers) to DIR/<name>.npy; --impl edb with --mode ddp/zero2/zero3 only; "
+                         "at N > 1 rank 0 writes its own loss and its local (zero2/zero3: sharded) "
+                         "state")
+    args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "edb" or args.mode == "auto"):
+        ap.error("--dump-outputs needs --impl edb and --mode ddp, zero2 or zero3")
+    return args
 
 
 def measured_peaks():
@@ -65,8 +78,9 @@ def measured_peaks():
             p = json.load(f)
         return {"bf16_tflops": p["bf16_tflops"], "bf16_tflops_sustained": p["bf16_tflops_sustained"],
                 "hbm_gbs": p["hbm_gbs"], "source": "measured (MEASURED_PEAKS.json)"}
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    # NVIDIA's H100 SXM data sheet (dense bf16, 700 W card): an upper bound, not a measured rate
+    return {"bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "hbm_gbs": 3350.0,
+            "source": "H100 SXM data sheet (dense bf16, 700 W)"}
 
 
 class ClockSampler:
@@ -165,7 +179,7 @@ def workload_config(args, world):
                         f"{args.batch_per_gpu} seq/GPU",
             "global_batch": args.batch_per_gpu * world, "seq_len": args.seq,
             "parallelism": f"{args.mode} dp{world}", "attention": args.attn,
-            "l2_policy": "per-step working set (weights+activations > 2 GB) exceeds the 126 MB L2",
+            "l2_policy": "per-step working set (weights+activations > 2 GB) exceeds the 50 MB L2",
             "cuda_graph": not args.no_cuda_graph}
 
 
@@ -173,7 +187,7 @@ def workload_config(args, world):
 
 
 def gemm_roofline(torch, gemm, calls, peaks, sustained, fused_calls=(), rank=0, pf_map=None):
-    """Dominant kernel = the tcgen05 GEMM.  Replays the step's GEMM launches (exact shapes, operand
+    """Dominant kernel = the wgmma GEMM.  Replays the step's GEMM launches (exact shapes, operand
     layouts and strides recorded from the compiled graph) back to back from a CUDA graph with CUDA
     events around the whole list on the launching stream; operands of consecutive launches differ
     and sum to far more than L2.  achieved = algorithmic FLOPs (2*M*N*K per launch) / measured time."""
@@ -264,16 +278,8 @@ def gemm_roofline(torch, gemm, calls, peaks, sustained, fused_calls=(), rank=0, 
     # the replay is a ~10-20 ms burst timed on its own, so the burst peak is the denominator
     # (the sustained figure is reported beside it)
     peak = peaks["bf16_tflops_sustained"] if sustained else peaks["bf16_tflops"]
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r02_gemm_dram_traffic.json")
-    if os.path.exists(tpath) and not fused_ops and not pf_map:
-        with open(tpath) as f:
-            traffic = json.load(f)
     return {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
             "frac": achieved / peak, "frac_of_sustained_peak": achieved / peaks["bf16_tflops_sustained"],
-            "traffic": (traffic or {}).get("dram_bytes_per_launch"),
-            "traffic_algorithmic_bytes_per_launch": (traffic or {}).get("algorithmic_bytes_per_launch"),
-            "traffic_source": (traffic or {}).get("source"),
             "kernel": "edb::k_gemm_bf16 (plain" + (", with all-gather prefetch CTAs" if pf_map else "")
                       + (", push-fused" if fused_ops else "") + ")",
             "launches_per_step": n_launch, "fused_launches_per_step": len(fused_ops),
@@ -283,6 +289,34 @@ def gemm_roofline(torch, gemm, calls, peaks, sustained, fused_calls=(), rank=0, 
             "cublas_same_launch_list_tflops": cublas_tf,
             "peak_source": peaks["source"] + (", sustained figure" if sustained else
                                               ", burst figure (the launch list is replayed on its own)")}
+
+
+DUMP_SAMPLE = 16384  # elements per tensor: ~300 tensors x 2 x 64 KiB stays far below 64 MB
+
+
+def dump_outputs(torch, out_dir, compiled, loss):
+    """The last step's results as float32 .npy files: `loss`, and for every parameter / momentum
+    buffer `param.<name>` / `momentum.<name>.<key>` — all elements, or DUMP_SAMPLE of them at
+    positions drawn from a generator seeded per tensor (the same positions in every run)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray(loss, dtype=np.float32))
+    params, _, named_states = compiled.get_state()
+
+    def save(name, t):
+        flat = t.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(sum(name.encode()))
+            idx = torch.randint(flat.numel(), (DUMP_SAMPLE,), generator=g).to(flat.device)
+            flat = flat[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), flat.float().cpu().numpy())
+
+    for n, p in params.items():
+        save(f"param.{n}", p)
+    for n, st in named_states.items():
+        for k, v in st.items():
+            if isinstance(v, torch.Tensor) and v.dim() > 0:
+                save(f"momentum.{n}.{k}", v)
 
 
 def parity_leg(torch, dist, args, cfg, GPT2, step_fn, model, opt, state0, par_host, first_loss,
@@ -448,6 +482,8 @@ def run_edb(args):
             dist.barrier()
         torch.cuda.synchronize()
 
+    loss_v_last = [None]
+
     def timed(n_steps, e2e):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         barrier()
@@ -465,6 +501,7 @@ def run_edb(args):
                 last = step_fn(t_d, y_d, model, opt)
         e1.record()
         barrier()
+        loss_v_last[0] = float(last)
         ms = torch.tensor([e0.elapsed_time(e1)], device="cuda")
         if world > 1:
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
@@ -485,6 +522,8 @@ def run_edb(args):
     ms_total, loss_v = timed(args.steps, e2e=False)
     clocks = sampler.stop() if rank == 0 else None
     ms_e2e, _ = timed(args.steps, e2e=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(torch, args.dump_outputs, step_fn.compiled_func, loss_v_last[0])
     errs = rt.error_flags()
     assert not any(errs), f"collective spin-wait timeouts: {errs}"
     gbatch = B * world
@@ -526,7 +565,7 @@ def run_edb(args):
         line["parity"] = parity
     if world > 1 and not args.no_parity:
         # the other half of BASELINE.json's metric: reshard bus bandwidth (nccl-tests convention)
-        # against NVLink-5 peak, 64 MiB bf16, push-protocol kernels vs NCCL on the same GPUs
+        # against the H100 SXM's NVLink-4 peak (450 GB/s per direction), 64 MiB bf16, push-protocol kernels vs NCCL on the same GPUs
         # (tests/mgpu_worker.py bench2: CUDA-graph timed, max over ranks; outside the timed region)
         try:
             from tests import mgpu_worker as W
@@ -535,13 +574,13 @@ def run_edb(args):
             r0 = next(r for r in rows if r["dim"] == "0")
             nb, f = r0["bytes"], (world - 1) / world
             line["reshard_bus"] = {
-                "bytes": nb, "dtype": "bf16", "unit": "GB/s", "nvlink_peak": 900.0,
+                "bytes": nb, "dtype": "bf16", "unit": "GB/s", "nvlink_peak": 450.0,
                 "all_gather": r0["ag_edb_GBs"], "reduce_scatter": r0["rs_edb_GBs"],
                 "all_reduce": r0.get("ar_edb_GBs"), "all_to_all": r0.get("a2a_edb_GBs"),
                 "nccl_all_gather": nb * f / r0["ag_nccl_us"] / 1e3,
                 "nccl_reduce_scatter": nb * f / r0["rs_nccl_us"] / 1e3,
                 "nccl_all_reduce": 2 * nb * f / r0["ar_nccl_us"] / 1e3 if "ar_nccl_us" in r0 else None,
-                "frac_of_nvlink_peak": r0["ag_edb_GBs"] / 900.0}
+                "frac_of_nvlink_peak": r0["ag_edb_GBs"] / 450.0}
         except Exception as e:  # the microbench must never sink the throughput line
             line["reshard_bus"] = {"error": repr(e)[:200]}
     if roof:

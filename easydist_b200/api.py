@@ -1,4 +1,4 @@
-"""`easydist_compile` for the B200 backend + registration behind the reference's own decorator.
+"""`easydist_compile` for the H100 backend + registration behind the reference's own decorator.
 
 Two ways in, both keeping the reference's user-facing contract (easydist/torch/api.py:227-256):
 

@@ -1,7 +1,7 @@
-"""Build libedb.so (the C-ABI CUDA runtime) in-tree for sm_100a.
+"""Build libedb.so (the C-ABI CUDA runtime) in-tree for sm_90a (H100).
 
 nvcc cross-compiles without a GPU, so this runs in the CPU container (`__graft_entry__.build()`)
-and the resulting .so travels to the GPU box with the repo snapshot.
+and the resulting .so is loaded from the source tree on the GPU machine.
 """
 import hashlib
 import os
@@ -20,9 +20,11 @@ BUILD_DIR = os.path.join(HERE, "csrc", "_build")
 HEADERS = ["edb_internal.cuh", "edb_vec.cuh"]
 SOURCES = ["edb_runtime.cu", "edb_reshard.cu", "edb_ll.cu", "edb_norm.cu", "edb_loss.cu", "edb_optim.cu", "edb_gemm.cu"]
 
+ARCH = "arch=compute_90a,code=sm_90a"
+
 NVCC_FLAGS = [
     "-std=c++17", "-O3", "-lineinfo",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", ARCH,
     "-Xcompiler", "-fPIC",
     "-I", INCLUDE, "-I", CSRC,
 ]
@@ -101,7 +103,7 @@ def _build_locked(verbose):
     if verbose:
         sys.stderr.write("\n".join(logs))
     tmp_lib = os.path.join(tmp, "libedb.so")
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", tmp_lib, *objs]
+    cmd = [nvcc, "-shared", "-gencode", ARCH, "-o", tmp_lib, *objs]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,20 +1,21 @@
-// Dense bf16 GEMM on Blackwell 5th-gen tensor cores (tcgen05 + TMEM + TMA), the compute half of
-// the sharded-op kernel dispatch: the aten.mm.default nodes of the sharded FX graph
+// Dense bf16 GEMM on Hopper tensor cores (wgmma + TMA + mbarrier), the compute half of the
+// sharded-op kernel dispatch: the aten.mm.default nodes of the sharded FX graph
 // (Linear fwd / dgrad / wgrad; SURVEY.md §8 a14) land here.
 //
-//   C[M,N] (bf16) = A · B, fp32 accumulation in tensor memory.
+//   C[M,N] (bf16) = A · B, fp32 accumulation in registers.
 //     A: K-major  ([M,K] row-major)  or MN-major (stored [K,M])
 //     B: K-major  ([N,K] row-major, i.e. nn.Linear weight) or MN-major (stored [K,N])
 //
-// Structure (one persistent CTA per SM, 192 threads):
-//   warp 0      : TMA producer   — cp.async.bulk.tensor tiles of A and B into a 4/6-stage smem ring
-//   warp 1      : MMA issuer     — one elected lane issues tcgen05.mma (128 x BN x 16), accumulators
-//                                  live in TMEM, double-buffered so the epilogue of tile i overlaps
-//                                  the main loop of tile i+1; also owns TMEM alloc/dealloc
-//   warps 2..5  : epilogue       — tcgen05.ld TMEM -> registers -> bf16 -> 16-byte global stores
-// Synchronisation is mbarrier-only (full/empty per smem stage, full/empty per TMEM stage).
+// Structure (one persistent CTA per SM, 288 threads):
+//   warps 0..7 : two consumer warpgroups — each issues wgmma.mma_async (64 x BN x 16) on its 64
+//                rows of the 128 x BN tile with the accumulator in registers, then runs the
+//                epilogue: registers -> bf16 -> 128B-swizzled smem -> TMA store
+//   warp 8     : TMA producer — one lane issues cp.async.bulk.tensor tiles of A and B into a
+//                4/6-stage smem ring, already loading the next tile while the consumers run the
+//                epilogue
+// Synchronisation is mbarrier-only (full/empty per smem stage).
 //
-// Shared-memory tiles use the canonical 128-byte-swizzle UMMA layouts, written by TMA with
+// Shared-memory tiles use the canonical 128-byte-swizzle wgmma layouts, written by TMA with
 // CU_TENSOR_MAP_SWIZZLE_128B and described to the tensor core with matching smem descriptors
 // (K-major: SBO = 1024 B; MN-major: one 64-element atom per TMA box, LBO = atom stride).
 #include <cuda.h>
@@ -26,19 +27,18 @@ namespace edb {
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 bf16 = 128 bytes = one swizzle atom
-constexpr int UMMA_K = 16;
-constexpr int kGemmThreads = 192;
+constexpr int MMA_K = 16;
+constexpr int kConsumerThreads = 256;                 // two warpgroups, 64 tile rows each
+constexpr int kGemmThreads = kConsumerThreads + 32;   // + the producer warp
 constexpr int kSmemABytes = BM * BK * 2;  // 16 KiB
 
-// CL = 1: one CTA computes a 128 x BN tile.  CL = 2: a CTA pair computes a 256 x BN tile with
-// tcgen05.mma.cta_group::2 — each CTA stages its own 128 rows of A and HALF of the B tile, so a
-// stage is 16 KiB + BN*64 B instead of 16 KiB + BN*128 B: more stages in flight (the 1-CTA kernel
-// is bound by TMA latency x stage depth: 62% tensor-pipe at 8192^3) and 1.5x less L2->SM traffic.
-template <int BN, int CL = 1> struct TileCfg {
-  static constexpr int kSmemBBytes = (BN / CL) * BK * 2;
+// A 128 x 256 tile reads 48 KiB of operands per 64-deep k-block for 2 x 64 x 256 x 64 MMAs, a
+// 128 x 128 tile 32 KiB for half the work: 256 wide whenever N allows.  Stages fill the 227 KiB an
+// H100 block may use (4 x 48 KiB or 6 x 32 KiB, + 32 KiB of epilogue staging).
+template <int BN> struct TileCfg {
+  static constexpr int kSmemBBytes = BN * BK * 2;
   static constexpr int kStageBytes = kSmemABytes + kSmemBBytes;
-  static constexpr int kStages = (CL == 2) ? ((BN == 256) ? 6 : 8) : ((BN == 256) ? 4 : 6);
-  static constexpr int kTmemCols = 2 * BN;  // two accumulator stages
+  static constexpr int kStages = (BN == 256) ? 4 : 6;
   static constexpr int kEpiBufBytes = BM * 64 * 2;  // one 128 x 64 bf16 store box (128B swizzle)
   static constexpr int kEpiBufs = 2;
   static constexpr int kSmemBytes =
@@ -76,6 +76,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t addr, uint32_t parity) {
 }
 // Spin on an mbarrier phase.  A watchdog turns a protocol bug into a trap (kernel error) instead
 // of a hung GPU: 4 s is ~1000x the longest legitimate wait of any role in these kernels.
+// No printf: it is a function call, and ptxas serialises the wgmmas of a kernel whose wgmma
+// pipeline may cross one.  The trap surfaces as a launch error on the host.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   const uint32_t addr = smem_u32(bar);
   if (mbar_try_wait(addr, parity)) return;
@@ -83,8 +85,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(addr, parity)) {
     if ((++spins & 0xfff) == 0 && globaltimer_ns() - t0 > 4000000000ull) {
-      printf("edb gemm watchdog: block %d thread %d stuck on barrier %u parity %u\n", blockIdx.x,
-             threadIdx.x, addr, parity);
       asm volatile("trap;");
     }
   }
@@ -120,156 +120,101 @@ __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 __device__ __forceinline__ void epi_bar_sync() {
-  asm volatile("bar.sync 1, 128;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_mcast(const CUtensorMap* map, uint64_t* bar, void* smem,
-                                                  int c0, int c1, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(smem)),
-      "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_mcast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%0], %1;" ::"r"(smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // shared::cluster address of the same offset in CTA rank 0
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* map, uint64_t* leader_bar,
-                                                void* smem, int c0, int c1) {
-  // executed by both CTAs of the pair; the transaction bytes update the LEADER's barrier
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];" ::"r"(smem_u32(smem)),
-      "l"(map), "r"(smem_u32(leader_bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void umma_f16_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                              uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 "
-      "[%0], %1;" ::"r"(smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_on_leader(uint64_t* bar) {
-  asm volatile(
-      "{\n"
-      ".reg .b32 raddr;\n"
-      "mapa.shared::cluster.u32 raddr, %0, 0;\n"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [raddr];\n"
-      "}\n" ::"r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols)
-               : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+  asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory");
 }
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
-__device__ __forceinline__ void tcgen05_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tcgen05_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+template <int N> __device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols)
-               : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                         uint32_t idesc, uint32_t accumulate) {
+
+// D[64 x N] (+)= A[64 x 16] · B[16 x N]; TA / TB = 1: operand stored MN-major (transposed).
+// scale_d == 0 starts a fresh accumulator.  The accumulator fragment of thread t of the warpgroup:
+// d[i] = D[16 (t / 32) + (t % 32) / 4 + 8 ((i / 2) % 2)][8 (i / 4) + 2 (t % 4) + i % 2].
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16(float* d, uint64_t desc_a, uint64_t desc_b,
+                                                  uint32_t scale_d) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, %67, %68;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n256k16(float* d, uint64_t desc_a, uint64_t desc_b,
+                                                  uint32_t scale_d) {
   asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1, %131, %132;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b), "r"(scale_d), "n"(TA), "n"(TB));
 }
 
 // ---- descriptors -------------------------------------------------------------------------------------
 
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout):
+// wgmma shared-memory matrix descriptor:
 //   [0,14) start address >> 4   [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4
-//   [46,48) version = 1 (sm_100)   [61,64) layout type: 2 = SWIZZLE_128B
+//   [49,52) base offset = 0 (tiles are 1024-byte aligned)   [62,64) layout type: 1 = SWIZZLE_128B
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes,
                                                    uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-
-// Instruction descriptor for kind::f16 (cute::UMMA::InstrDescriptor bit layout):
-//   [4,6) D format: 1 = F32   [7,10) A format: 1 = BF16   [10,13) B format: 1 = BF16
-//   [15] A major: 0 = K, 1 = MN   [16] B major   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc(int m, int n, bool a_mn, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-         ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
 }
 
 struct GemmParams {
@@ -436,10 +381,7 @@ __device__ __forceinline__ void spin_wait_gpu(const uint64_t* flag, uint64_t tar
   uint32_t spins = 0;
   while (ld_acquire_gpu(flag) < target) {
     __nanosleep(32);
-    if ((++spins & 0xfff) == 0 && globaltimer_ns() - t0 > 4000000000ull) {
-      printf("edb fused gemm watchdog: block %d stuck on chunk flag\n", blockIdx.x);
-      asm volatile("trap;");
-    }
+    if ((++spins & 0xfff) == 0 && globaltimer_ns() - t0 > 4000000000ull) asm volatile("trap;");
   }
 }
 
@@ -751,18 +693,30 @@ __device__ __forceinline__ void rs_tail_reduce(const FusedArgs& fa, uint64_t tid
 
 // ---- kernel ------------------------------------------------------------------------------------------
 
-// CL = 2: thread-block cluster of two CTAs = one 256 x BN tile computed with cta_group::2 UMMA.
-// Both CTAs run the TMA producer (own 128 rows of A + own half of B, transaction bytes counted on
-// the leader's `full` barrier) and the epilogue (own 128 accumulator rows in own TMEM); only the
-// leader (cluster rank 0) issues the MMAs and multicasts `commit` to both CTAs' barriers.
-// (A multicast-only variant of this cluster shape was measured first: +4%, TMA multicast does not
-// save L2 reads at cluster size 2 — profiles/r01_gemm_vs_cublas_v3_cluster_multicast.log.)
-template <int BN, bool A_KMAJOR, bool B_KMAJOR, int MODE, int CL>
+// One consumer warpgroup's accumulator: rows 64 wg + [0, 64) of the tile, all BN columns.
+// Epilogue helpers below address it through the fragment layout of wgmma_m64n*k16.
+template <int BN, bool A_KMAJOR, bool B_KMAJOR>
+__device__ __forceinline__ void mma_k_block(float* acc, uint32_t a_addr, uint32_t b_addr, bool fresh) {
+#pragma unroll
+  for (int k = 0; k < BK / MMA_K; ++k) {
+    // K-major: the 16-element k step moves 32 bytes inside the 128-byte swizzle row;
+    // MN-major: it moves 16 k rows of 128 bytes
+    const uint64_t da = A_KMAJOR ? make_smem_desc(a_addr + k * MMA_K * 2, 16, 1024)
+                                 : make_smem_desc(a_addr + k * MMA_K * 128, 64 * BK * 2, 1024);
+    const uint64_t db = B_KMAJOR ? make_smem_desc(b_addr + k * MMA_K * 2, 16, 1024)
+                                 : make_smem_desc(b_addr + k * MMA_K * 128, 64 * BK * 2, 1024);
+    const uint32_t scale_d = (fresh && k == 0) ? 0u : 1u;
+    if (BN == 256) wgmma_m64n256k16<A_KMAJOR ? 0 : 1, B_KMAJOR ? 0 : 1>(acc, da, db, scale_d);
+    else wgmma_m64n128k16<A_KMAJOR ? 0 : 1, B_KMAJOR ? 0 : 1>(acc, da, db, scale_d);
+  }
+}
+
+template <int BN, bool A_KMAJOR, bool B_KMAJOR, int MODE>
 __global__ void __launch_bounds__(kGemmThreads, 1)
     k_gemm_bf16(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                 const __grid_constant__ CUtensorMap tmap_c, const GemmParams p,
                 const __grid_constant__ FusedArgs fa, const __grid_constant__ CMaps cm) {
-  using Cfg = TileCfg<BN, CL>;
+  using Cfg = TileCfg<BN>;
   constexpr int kStages = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -803,7 +757,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
     }
   }
   if (MODE == MODE_PLAIN && fa.pf_ctas > 0 && (int)blockIdx.x < fa.pf_ctas) {
-    // prefetch CTAs (whole clusters when CL == 2): lowest block indices, no part in the GEMM
+    // prefetch CTAs: lowest block indices, no part in the GEMM
     pf_role(fa, smem, (int)blockIdx.x, fa.pf_ctas);
     return;
   }
@@ -816,55 +770,31 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_epi + Cfg::kEpiBufs * Cfg::kEpiBufBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
-  uint64_t* tmem_full = bars + 2 * kStages;
-  uint64_t* tmem_empty = bars + 2 * kStages + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 4);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int k_blocks = (p.K + BK - 1) / BK;
-  // work units: single tiles (CL == 1) or vertical tile pairs handled by one cluster (CL == 2)
-  const int crank = (CL == 2) ? (int)cluster_ctarank() : 0;
-  const int pm_tiles = (CL == 2) ? (p.m_tiles + 1) / 2 : p.m_tiles;
-  const int num_tiles = pm_tiles * p.n_tiles;
+  const int num_tiles = p.m_tiles * p.n_tiles;
   const int num_units = (MODE == MODE_PLAIN) ? num_tiles * p.splits : num_tiles;
-  const int unit0 = (CL == 2) ? cta / 2 : cta;
-  const int unit_stride = (CL == 2) ? n_gemm_ctas / 2 : n_gemm_ctas;
 
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmap_a);
-    prefetch_tmap(&tmap_b);
-    prefetch_tmap(&tmap_c);
-  }
-  if (warp == 1) {
-    if (lane == 0) {
-      for (int s = 0; s < kStages; ++s) {
-        mbar_init(&full_bar[s], 1);
-        mbar_init(&empty_bar[s], 1);
-      }
-      for (int s = 0; s < 2; ++s) {
-        mbar_init(&tmem_full[s], 1);
-        mbar_init(&tmem_empty[s], 4 * CL);  // one arrive per epilogue warp (of both CTAs if CL == 2)
-      }
-      fence_barrier_init();
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
     }
-    __syncwarp();
-    if (CL == 2) tmem_alloc_2cta(tmem_slot, Cfg::kTmemCols);
-    else tmem_alloc(tmem_slot, Cfg::kTmemCols);
+    fence_barrier_init();
   }
-  tcgen05_fence_before();
   __syncthreads();
-  if (CL == 2) cluster_sync_all();  // the peer's barriers exist before anything is multicast at them
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == kConsumerThreads / 32) {
     // ===== TMA producer =====
     if (lane == 0) {
+      prefetch_tmap(&tmap_a);
+      prefetch_tmap(&tmap_b);
       int stage = 0;
       uint32_t phase = 0;
       int ready_chunk = -1;
-      for (int u = unit0; u < num_units; u += unit_stride) {
+      for (int u = cta; u < num_units; u += n_gemm_ctas) {
         const int t = (MODE == MODE_PLAIN) ? u % num_tiles : u;
         int kb0 = 0, kb1 = k_blocks;
         if (MODE == MODE_PLAIN && p.splits > 1) {
@@ -872,13 +802,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
           kb1 = kb0 + p.kb_per_split < k_blocks ? kb0 + p.kb_per_split : k_blocks;
         }
         int m_blk, n_blk, chunk;
-        if (CL == 2) {
-          chunk = 0;
-          m_blk = 2 * ((t % pm_tiles + p.m_rot) % pm_tiles) + crank;
-          n_blk = t / pm_tiles;
-        } else {
-          tile_coords<MODE>(t, p, fa, m_blk, n_blk, chunk);
-        }
+        tile_coords<MODE>(t, p, fa, m_blk, n_blk, chunk);
         const CUtensorMap* bmap = &tmap_b;
         int b_row = n_blk * BN;
         if (MODE == MODE_AG) {
@@ -897,32 +821,6 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem_a + stage * kSmemABytes;
           uint8_t* sb = smem_b + stage * Cfg::kSmemBBytes;
-          if (CL == 2) {
-            // both CTAs' loads complete on the leader's barrier, which expects both stages' bytes
-            if (crank == 0) mbar_expect_tx(&full_bar[stage], 2 * Cfg::kStageBytes);
-            if (A_KMAJOR) {
-              tma_load_2d_2sm(&tmap_a, &full_bar[stage], sa, kb * BK, m_blk * BM);
-            } else {
-#pragma unroll
-              for (int h = 0; h < BM / 64; ++h)
-                tma_load_2d_2sm(&tmap_a, &full_bar[stage], sa + h * (64 * BK * 2),
-                                m_blk * BM + h * 64, kb * BK);
-            }
-            const int b_half = b_row + crank * (BN / 2);
-            if (B_KMAJOR) {
-              tma_load_2d_2sm(bmap, &full_bar[stage], sb, kb * BK, b_half);
-            } else {
-#pragma unroll
-              for (int h = 0; h < BN / 128; ++h)
-                tma_load_2d_2sm(bmap, &full_bar[stage], sb + h * (64 * BK * 2), b_half + h * 64,
-                                kb * BK);
-            }
-            if (++stage == kStages) {
-              stage = 0;
-              phase ^= 1;
-            }
-            continue;
-          }
           mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
           if (A_KMAJOR) {
             tma_load_2d(&tmap_a, &full_bar[stage], sa, kb * BK, m_blk * BM);
@@ -947,112 +845,63 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         }
       }
     }
-  } else if (warp == 1 && (CL == 1 || crank == 0)) {
-    // ===== MMA issuer (leader CTA only when CL == 2) =====
-    constexpr uint32_t idesc = make_idesc(BM * CL, BN, !A_KMAJOR, !B_KMAJOR);
+  } else {
+    // ===== consumer warpgroups: wgmma main loop, then registers -> bf16 -> swizzled smem -> TMA store
+    const int wg = warp >> 2;
+    const int tid = threadIdx.x & 127;
+    const int frag_row = 16 * (tid >> 5) + ((tid & 31) >> 2);  // + 8 for the odd register pairs
+    const int frag_col = 2 * (tid & 3);
+    const int row0 = wg * 64 + frag_row;                       // tile row of h = 0
+    const bool issuer = (threadIdx.x == 0);
+    if (issuer) prefetch_tmap(&tmap_c);
+    float acc[BN / 2];
     int stage = 0;
     uint32_t phase = 0;
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int u = unit0; u < num_units; u += unit_stride) {
+    int ebuf = 0;
+    for (int u = cta; u < num_units; u += n_gemm_ctas) {
+      const int t = (MODE == MODE_PLAIN) ? u % num_tiles : u;
       int kb0 = 0, kb1 = k_blocks;
       if (MODE == MODE_PLAIN && p.splits > 1) {
         kb0 = (u / num_tiles) * p.kb_per_split;
         kb1 = kb0 + p.kb_per_split < k_blocks ? kb0 + p.kb_per_split : k_blocks;
       }
-      mbar_wait(&tmem_empty[as], aphase ^ 1);
-      tcgen05_fence_after();
-      const uint32_t tmem_d = tmem_base + as * BN;
+      int m_blk, n_blk, chunk;
+      tile_coords<MODE>(t, p, fa, m_blk, n_blk, chunk);
+
+      // main loop: one wgmma group in flight; a stage goes back to the producer once the group
+      // that read it has retired
+      int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        tcgen05_fence_after();
-        if (lane == 0) {
-          const uint32_t a_addr = smem_u32(smem_a + stage * kSmemABytes);
-          const uint32_t b_addr = smem_u32(smem_b + stage * Cfg::kSmemBBytes);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) {
-            uint64_t da, db;
-            if (A_KMAJOR) da = make_smem_desc(a_addr + k * UMMA_K * 2, 0, 1024);
-            else da = make_smem_desc(a_addr + k * UMMA_K * 128, 64 * BK * 2, 1024);
-            if (B_KMAJOR) db = make_smem_desc(b_addr + k * UMMA_K * 2, 0, 1024);
-            else db = make_smem_desc(b_addr + k * UMMA_K * 128, 64 * BK * 2, 1024);
-            if (CL == 2) umma_f16_2cta(tmem_d, da, db, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            else umma_f16(tmem_d, da, db, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          // free the smem stage when these MMAs retire (in both CTAs of a pair)
-          if (CL == 2) {
-            umma_commit_2cta(&empty_bar[stage], (uint16_t)3);
-            if (kb == kb1 - 1) umma_commit_2cta(&tmem_full[as], (uint16_t)3);
-          } else {
-            umma_commit(&empty_bar[stage]);
-            if (kb == kb1 - 1) umma_commit(&tmem_full[as]);
-          }
-        }
-        __syncwarp();
+        wgmma_fence();
+        mma_k_block<BN, A_KMAJOR, B_KMAJOR>(acc, smem_u32(smem_a + stage * kSmemABytes) + wg * (64 * BK * 2),
+                                            smem_u32(smem_b + stage * Cfg::kSmemBBytes), kb == kb0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
         if (++stage == kStages) {
           stage = 0;
           phase ^= 1;
         }
       }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
-    }
-  } else if (warp >= 2) {
-    // ===== epilogue warps 2..5: TMEM -> registers -> bf16 -> swizzled smem -> TMA store =====
-    const int quad = warp & 3;            // TMEM lane quadrant this warp may access
-    const int row_in_tile = quad * 32 + lane;
-    const bool issuer = (warp == 2 && lane == 0);
-    int as = 0;
-    uint32_t aphase = 0;
-    int ebuf = 0;
-    for (int u = unit0; u < num_units; u += unit_stride) {
-      const int t = (MODE == MODE_PLAIN) ? u % num_tiles : u;
-      int m_blk, n_blk, chunk;
-      if (CL == 2) {
-        chunk = 0;
-        m_blk = 2 * ((t % pm_tiles + p.m_rot) % pm_tiles) + crank;
-        n_blk = t / pm_tiles;
-      } else {
-        tile_coords<MODE>(t, p, fa, m_blk, n_blk, chunk);
-      }
+      wgmma_wait<0>();
+      if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+
       if (MODE == MODE_PLAIN && p.splits > 1) {
-        // split-K: this unit's fp32 partial goes straight from registers to the workspace (one
-        // 256-byte run per thread and chunk); k_splitk_reduce adds the slices, bias and rounds
-        mbar_wait(&tmem_full[as], aphase);
-        tcgen05_fence_after();
-        const int64_t r = (int64_t)m_blk * BM + row_in_tile;
-        float* prow = p.partial + ((int64_t)(u / num_tiles) * p.M + r) * p.ldp;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 64) {
-          uint32_t v[64];
-          const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * BN + c0);
-          tmem_ld_32x32b_x32(taddr, v);
-          tmem_ld_32x32b_x32(taddr + 32, v + 32);
-          tmem_ld_wait();
-          if (c0 + 64 >= BN) {
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-              if (CL == 2) mbar_arrive_on_leader(&tmem_empty[as]);
-              else mbar_arrive(&tmem_empty[as]);
-            }
-          }
-          const int col0 = n_blk * BN + c0;
-          if (r < p.M) {
+        // split-K: this unit's fp32 partial goes straight from registers to the workspace;
+        // k_splitk_reduce adds the slices and the bias, and rounds
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int col = col0 + 4 * j;
-              if (col < p.ldp)  // ldp = N rounded up to 4: whole float4 groups only
-                *reinterpret_cast<uint4*>(prow + col) =
-                    make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-            }
+        for (int h = 0; h < 2; ++h) {
+          const int64_t r = (int64_t)m_blk * BM + row0 + 8 * h;
+          if (r >= p.M) continue;
+          float* prow = p.partial + ((int64_t)(u / num_tiles) * p.M + r) * p.ldp;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int col = n_blk * BN + 8 * j + frag_col;
+            if (col < p.ldp)  // ldp = N rounded up to 4, col even: whole float2 pairs only
+              *reinterpret_cast<float2*>(prow + col) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
           }
-        }
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1;
         }
         continue;
       }
@@ -1067,76 +916,36 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         cmap = &cm.m[owner];
         c_row = (m_blk - owner * p.push_mtc) * BM;
       }
-      // fused elementwise epilogue: this thread's 64 aux values of a chunk (one 128-byte row
-      // segment) are requested one chunk AHEAD — the first one before the accumulator is even
-      // complete — so that their latency hides behind the main loop / the previous chunk
       const bool has_aux = (MODE == MODE_PLAIN && p.epi_op != EPI_NONE);
-      const int64_t arow_i = (int64_t)m_blk * BM + row_in_tile;
-      const __nv_bfloat16* arow = has_aux ? p.aux + arow_i * p.ld_aux + (int64_t)n_blk * BN : nullptr;
-      uint4 anext[8];
-      auto load_aux = [&](int c0) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          if (arow_i < p.M && n_blk * BN + c0 + 8 * j < p.N)
-            anext[j] = __ldg(reinterpret_cast<const uint4*>(arow + c0 + 8 * j));
-          else
-            anext[j] = make_uint4(0, 0, 0, 0);
-        }
-      };
-      if (has_aux) load_aux(0);
-      mbar_wait(&tmem_full[as], aphase);
-      tcgen05_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 64) {
-        uint32_t v[64];
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * BN + c0);
-        tmem_ld_32x32b_x32(taddr, v);
-        tmem_ld_32x32b_x32(taddr + 32, v + 32);
-        uint4 acur[8];
-        if (has_aux) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) acur[j] = anext[j];
-          if (c0 + 64 < BN) load_aux(c0 + 64);
-        }
-        tmem_ld_wait();
-        if (c0 + 64 >= BN) {
-          // all of this warp's accumulator columns are in registers: hand the TMEM stage back
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            if (CL == 2) mbar_arrive_on_leader(&tmem_empty[as]);
-            else mbar_arrive(&tmem_empty[as]);
-          }
-        }
-        // the staging buffer we are about to overwrite must have been read by its TMA store
-        if (issuer) tma_store_wait_read<Cfg::kEpiBufs - 1>();
-        epi_bar_sync();
-        uint8_t* buf = smem_epi + ebuf * Cfg::kEpiBufBytes;
-        uint8_t* rowp = buf + row_in_tile * 128;
+      for (int c0 = 0; c0 < BN; c0 += 64) {  // unrolled: acc must only ever be indexed statically
+        float* v = acc + c0 / 2;  // this thread's 32 values of columns [c0, c0 + 64)
         if (p.bias != nullptr) {
-          const int col0 = n_blk * BN + c0;
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
-            if (col0 + 8 * j < p.N) {  // N % 8 == 0 whenever a bias is passed
-              const uint4 braw = __ldg(reinterpret_cast<const uint4*>(p.bias + col0 + 8 * j));
-              const __nv_bfloat162* bb = reinterpret_cast<const __nv_bfloat162*>(&braw);
+            const int col = n_blk * BN + c0 + 8 * j + frag_col;
+            if (col < p.N) {  // N % 8 == 0 whenever a bias is passed
+              const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.bias + col));
 #pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float2 f = __bfloat1622float2(bb[e]);
-                v[8 * j + 2 * e] = __float_as_uint(__uint_as_float(v[8 * j + 2 * e]) + f.x);
-                v[8 * j + 2 * e + 1] = __float_as_uint(__uint_as_float(v[8 * j + 2 * e + 1]) + f.y);
+              for (int h = 0; h < 2; ++h) {
+                v[4 * j + 2 * h] += f.x;
+                v[4 * j + 2 * h + 1] += f.y;
               }
             }
           }
         }
         if (has_aux) {
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const __nv_bfloat162* aa = reinterpret_cast<const __nv_bfloat162*>(&acur[j]);
+          for (int h = 0; h < 2; ++h) {
+            const int64_t r = (int64_t)m_blk * BM + row0 + 8 * h;
+            const __nv_bfloat16* arow = p.aux + r * p.ld_aux;
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float2 f = __bfloat1622float2(aa[e]);
-              float x0 = __uint_as_float(v[8 * j + 2 * e]), x1 = __uint_as_float(v[8 * j + 2 * e + 1]);
+            for (int j = 0; j < 8; ++j) {
+              const int col = n_blk * BN + c0 + 8 * j + frag_col;
+              float2 f = make_float2(0.f, 0.f);
+              if (r < p.M && col < p.N)
+                f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(arow + col));
+              float x0 = v[4 * j + 2 * h], x1 = v[4 * j + 2 * h + 1];
               if (p.epi_op == EPI_ADD) {
                 x0 += f.x;
                 x1 += f.y;
@@ -1145,24 +954,25 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
                 x0 = __bfloat162float(__float2bfloat16_rn(x0)) * gelu_tanh_grad(f.x);
                 x1 = __bfloat162float(__float2bfloat16_rn(x1)) * gelu_tanh_grad(f.y);
               }
-              v[8 * j + 2 * e] = __float_as_uint(x0);
-              v[8 * j + 2 * e + 1] = __float_as_uint(x1);
+              v[4 * j + 2 * h] = x0;
+              v[4 * j + 2 * h + 1] = x1;
             }
           }
         }
+        // the staging buffer we are about to overwrite must have been read by its TMA store
+        if (issuer) tma_store_wait_read<Cfg::kEpiBufs - 1>();
+        epi_bar_sync();
+        uint8_t* buf = smem_epi + ebuf * Cfg::kEpiBufBytes;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          uint4 o;
-          __nv_bfloat162 h0 = __floats2bfloat162_rn(__uint_as_float(v[8 * j + 0]), __uint_as_float(v[8 * j + 1]));
-          __nv_bfloat162 h1 = __floats2bfloat162_rn(__uint_as_float(v[8 * j + 2]), __uint_as_float(v[8 * j + 3]));
-          __nv_bfloat162 h2 = __floats2bfloat162_rn(__uint_as_float(v[8 * j + 4]), __uint_as_float(v[8 * j + 5]));
-          __nv_bfloat162 h3 = __floats2bfloat162_rn(__uint_as_float(v[8 * j + 6]), __uint_as_float(v[8 * j + 7]));
-          o.x = *reinterpret_cast<uint32_t*>(&h0);
-          o.y = *reinterpret_cast<uint32_t*>(&h1);
-          o.z = *reinterpret_cast<uint32_t*>(&h2);
-          o.w = *reinterpret_cast<uint32_t*>(&h3);
-          // 128-byte swizzle: 16-byte chunk j of row r lives at chunk (j ^ (r & 7))
-          *reinterpret_cast<uint4*>(rowp + ((j ^ (row_in_tile & 7)) << 4)) = o;
+        for (int h = 0; h < 2; ++h) {
+          const int row = row0 + 8 * h;
+          uint8_t* rowp = buf + row * 128 + frag_col * 2;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            __nv_bfloat162 o = __floats2bfloat162_rn(v[4 * j + 2 * h], v[4 * j + 2 * h + 1]);
+            // 128-byte swizzle: 16-byte chunk j of row r lives at chunk (j ^ (r & 7))
+            *reinterpret_cast<__nv_bfloat162*>(rowp + ((j ^ (row & 7)) << 4)) = o;
+          }
         }
         fence_proxy_async();
         epi_bar_sync();
@@ -1178,17 +988,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
         tma_store_wait_all();
         fence_proxy_async_all();
         __threadfence_system();
-        const unsigned long long prev = atomicAdd(
+        const unsigned long long prev_cnt = atomicAdd(
             reinterpret_cast<unsigned long long*>(fa.f.local + F_TILECNT + chunk), 1ULL);
-        if (prev == (unsigned long long)fa.tiles_per_chunk - 1) {
+        if (prev_cnt == (unsigned long long)fa.tiles_per_chunk - 1) {
           fa.f.local[F_TILECNT + chunk] = 0;
           __threadfence_system();
           st_release_sys(fa.f.peer[chunk] + (fa.rs_defer ? F_PUSHED : F_CHUNK) + fa.f.me, q);
         }
-      }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
       }
     }
     if (issuer) {
@@ -1206,16 +1012,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
     }
   }
 
-  tcgen05_fence_before();
-  __syncthreads();
-  if (CL == 2) cluster_sync_all();  // nobody leaves while the peer may still signal its barriers
-  if (warp == 1) {
-    tcgen05_fence_after();
-    if (CL == 2) tmem_dealloc_2cta(tmem_base, Cfg::kTmemCols);
-    else tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
-
   if (MODE == MODE_RS) {
+    __syncthreads();
     if (fa.rs_defer) {
       if (blockIdx.x == 0 && threadIdx.x == 0) fa.rs_state[0] = q;  // read by k_rs_finish (later kernel)
     } else {
@@ -1442,71 +1240,42 @@ static int make_tmap(CUtensorMap* map, const void* base, int64_t inner, int64_t 
   return EDB_OK;
 }
 
-template <int BN, bool AK, bool BK_, int MODE, int CL>
-static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
-                          const GemmParams& p, const FusedArgs& fa, const CMaps& cm, int grid,
-                          cudaStream_t st) {
-  using Cfg = TileCfg<BN, CL>;
+template <int BN, bool AK, bool BK_, int MODE>
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
+                       const GemmParams& p, const FusedArgs& fa, const CMaps& cm, int grid,
+                       cudaStream_t st) {
+  using Cfg = TileCfg<BN>;
   static bool configured = false;
-  auto kern = k_gemm_bf16<BN, AK, BK_, MODE, CL>;
+  auto kern = k_gemm_bf16<BN, AK, BK_, MODE>;
   if (!configured) {
     EDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     configured = true;
   }
-  if (CL == 1) {
-    kern<<<grid, kGemmThreads, Cfg::kSmemBytes, st>>>(ta, tb, tc, p, fa, cm);
-  } else {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kGemmThreads);
-    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CL;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    EDB_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, tc, p, fa, cm));
-  }
+  kern<<<grid, kGemmThreads, Cfg::kSmemBytes, st>>>(ta, tb, tc, p, fa, cm);
   count_launch();
   return cuda_check(cudaGetLastError(), "k_gemm_bf16 launch");
-}
-
-template <int BN, bool AK, bool BK_, int MODE>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
-                       const GemmParams& p, const FusedArgs& fa, const CMaps& cm, int grid,
-                       cudaStream_t st, int cl = 1) {
-  if (MODE == MODE_PLAIN && cl == 2)
-    return launch_gemm_cl<BN, AK, BK_, MODE_PLAIN, 2>(ta, tb, tc, p, fa, cm, grid, st);
-  return launch_gemm_cl<BN, AK, BK_, MODE, 1>(ta, tb, tc, p, fa, cm, grid, st);
 }
 
 template <int MODE>
 static int dispatch_gemm(int bn, bool a_k, bool b_k, const CUtensorMap& ta, const CUtensorMap& tb,
                          const CUtensorMap& tc, const GemmParams& p, const FusedArgs& fa,
-                         const CMaps& cm, int grid, cudaStream_t st, int cl = 1) {
+                         const CMaps& cm, int grid, cudaStream_t st) {
   const int key = (bn == 256 ? 4 : 0) | (a_k ? 2 : 0) | (b_k ? 1 : 0);
   switch (key) {
-    case 7: return launch_gemm<256, true, true, MODE>(ta, tb, tc, p, fa, cm, grid, st, cl);
-    case 6: return launch_gemm<256, true, false, MODE>(ta, tb, tc, p, fa, cm, grid, st, cl);
-    case 5: return launch_gemm<256, false, true, MODE>(ta, tb, tc, p, fa, cm, grid, st, cl);
-    case 4: return launch_gemm<256, false, false, MODE>(ta, tb, tc, p, fa, cm, grid, st, cl);
-    case 3: return launch_gemm<128, true, true, MODE>(ta, tb, tc, p, fa, cm, grid, st, cl);
-    case 2: return launch_gemm<128, true, false, MODE>(ta, tb, tc, p, fa, cm, grid, st, cl);
-    case 1: return launch_gemm<128, false, true, MODE>(ta, tb, tc, p, fa, cm, grid, st, cl);
-    default: return launch_gemm<128, false, false, MODE>(ta, tb, tc, p, fa, cm, grid, st, cl);
+    case 7: return launch_gemm<256, true, true, MODE>(ta, tb, tc, p, fa, cm, grid, st);
+    case 6: return launch_gemm<256, true, false, MODE>(ta, tb, tc, p, fa, cm, grid, st);
+    case 5: return launch_gemm<256, false, true, MODE>(ta, tb, tc, p, fa, cm, grid, st);
+    case 4: return launch_gemm<256, false, false, MODE>(ta, tb, tc, p, fa, cm, grid, st);
+    case 3: return launch_gemm<128, true, true, MODE>(ta, tb, tc, p, fa, cm, grid, st);
+    case 2: return launch_gemm<128, true, false, MODE>(ta, tb, tc, p, fa, cm, grid, st);
+    case 1: return launch_gemm<128, false, true, MODE>(ta, tb, tc, p, fa, cm, grid, st);
+    default: return launch_gemm<128, false, false, MODE>(ta, tb, tc, p, fa, cm, grid, st);
   }
 }
 
-static int pick_bn(int64_t M, int64_t N, int sms) {
-  // 128-wide tiles need 128 B/cycle of operand traffic per SM (A 16 KiB + B 16 KiB per 256 MMA
-  // cycles) and run at ~half the rate of 256-wide ones (96 B/cycle) even when they quantise better
-  // into waves (measured: profiles/r01_gemm_tile_cluster_sweep.log), so 256 unless N is tiny.
-  (void)M;
-  (void)sms;
+static int pick_bn(int64_t N) {
+  // 256-wide tiles halve the A traffic per MMA (see TileCfg); 128 only where N leaves nothing
+  // for the second half of a 256-wide tile
   return N <= 128 ? 128 : 256;
 }
 
@@ -1561,7 +1330,7 @@ static float* splitk_workspace(cudaStream_t st) {
 static int sm_count_now() {
   Runtime& r = rt();
   if (!r.inited) {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess)
       cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     r.sm_count = sms;
@@ -1635,8 +1404,7 @@ static int fill_prefetch(FusedArgs* fa, const PfSpec* pf, int want_ctas) {
   }
   int ctas = want_ctas;
   if (blocks < ctas) ctas = (int)blocks;
-  ctas &= ~1;  // whole clusters when the GEMM runs CTA pairs
-  if (ctas < 2 && blocks > 0) ctas = 2;
+  if (ctas < 1 && blocks > 0) ctas = 1;
   fa->pf_ctas = pf->n_items > 0 ? ctas : 0;
   return EDB_OK;
 }
@@ -1648,17 +1416,13 @@ static int gemm_plain_impl(void* C, const void* A, const void* B, const void* bi
   int rc = check_operands(A, B, C, bias, M, N, K, lda, ldb, ldc, "edb_gemm_bf16");
   if (rc) return rc;
   const int sms = sm_count_now();
-  int bn = pick_bn(M, N, sms);
+  int bn = pick_bn(N);
   if (rt().gemm_force_bn == 128 || rt().gemm_force_bn == 256) bn = (int)rt().gemm_force_bn;
-  // CTA pairs (cta_group::2) whenever there are at least two tile rows (push: an even number, so
-  // that no pair has a phantom tile whose owner index would be out of range)
-  int cl = (rt().gemm_cluster >= 2 && M > BM) ? 2 : 1;
-  if (push && ((M / BM) & 1)) cl = 1;
   CUtensorMap ta, tb, tc;
   if (a_kmajor) rc = make_tmap(&ta, A, K, M, lda, BK, BM);
   else rc = make_tmap(&ta, A, M, K, lda, 64, BK);
   if (rc) return rc;
-  if (b_kmajor) rc = make_tmap(&tb, B, K, N, ldb, BK, bn / cl);
+  if (b_kmajor) rc = make_tmap(&tb, B, K, N, ldb, BK, bn);
   else rc = make_tmap(&tb, B, N, K, ldb, 64, BK);
   if (rc) return rc;
   rc = make_tmap(&tc, C, N, push ? push->rows_per : M, ldc, 64, BM);
@@ -1709,7 +1473,7 @@ static int gemm_plain_impl(void* C, const void* A, const void* B, const void* bi
     p.push_mtc = (int)(push->rows_per / BM);
     // start with the rows of the next member, end with my own (a local store)
     const int first_m = ((push->me + 1) % push->n) * p.push_mtc;
-    p.m_rot = (cl == 2) ? first_m / 2 : first_m;
+    p.m_rot = first_m;
     pd.n = push->n;
     pd.rows_per = push->rows_per;
     pd.row_rot = (int64_t)first_m * BM;
@@ -1727,8 +1491,8 @@ static int gemm_plain_impl(void* C, const void* A, const void* B, const void* bi
   // split-K: when the tiles occupy at most half of the SMs and K is long (weight gradients:
   // M, N = layer widths, K = tokens), slices of K go to the idle SMs.  Each slice keeps >= 8
   // k-blocks so that the pipeline fill and the fp32 partial traffic stay small against the MMAs.
-  const int units = (cl == 2 ? ((p.m_tiles + 1) / 2) : p.m_tiles) * p.n_tiles;
-  const int ctas = units * cl;
+  const int units = p.m_tiles * p.n_tiles;
+  const int ctas = units;
   const int k_blocks = (int)((K + BK - 1) / BK);
   if (rt().gemm_splitk && 2 * ctas <= sms_gemm && k_blocks >= 16 && p.epi_op == EPI_NONE) {
     int splits = sms_gemm / ctas;
@@ -1745,17 +1509,10 @@ static int gemm_plain_impl(void* C, const void* A, const void* B, const void* bi
       }
     }
   }
-  int grid;
-  if (cl == 2) {
-    const int pairs = units * p.splits;
-    const int clusters = pairs < sms_gemm / 2 ? pairs : sms_gemm / 2;
-    grid = 2 * clusters;
-  } else {
-    const int tiles = units * p.splits;
-    grid = tiles < sms_gemm ? tiles : sms_gemm;
-  }
+  const int tiles = units * p.splits;
+  int grid = tiles < sms_gemm ? tiles : sms_gemm;
   grid += fa.pf_ctas;
-  rc = dispatch_gemm<MODE_PLAIN>(bn, a_kmajor != 0, b_kmajor != 0, ta, tb, tc, p, fa, cm, grid, st, cl);
+  rc = dispatch_gemm<MODE_PLAIN>(bn, a_kmajor != 0, b_kmajor != 0, ta, tb, tc, p, fa, cm, grid, st);
   if (rc || p.splits == 1) return rc;
   const int64_t groups = (int64_t)M * (p.ldp / 4);
   int rgrid = (int)((groups + 255) / 256);
@@ -2058,7 +1815,7 @@ static int gemm_rs_impl(int gid, void* dst, uint64_t recv_off, uint64_t state_of
   rc = check_operands(A, B, recv, nullptr, M, N, K, lda, ldb, N, "edb_gemm_rs_bf16");
   if (rc) return rc;
   const int sms = r.sm_count;
-  const int bn = pick_bn(M, N, sms);
+  const int bn = pick_bn(N);
   CUtensorMap ta, tb, tc;
   if (a_kmajor) rc = make_tmap(&ta, A, K, M, lda, BK, BM);
   else rc = make_tmap(&ta, A, M, K, lda, 64, BK);

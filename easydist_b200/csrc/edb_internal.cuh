@@ -69,7 +69,7 @@ struct Group {
 
 struct Runtime {
   bool inited = false;
-  int rank = 0, world = 1, device = 0, sm_count = 148;
+  int rank = 0, world = 1, device = 0, sm_count = 132;
   char* heap = nullptr;
   size_t heap_bytes = 0;
   size_t bump = kUserOffset;
@@ -88,7 +88,6 @@ struct Runtime {
   int64_t gemm_force_bn = 0;  // tuning aid: 128 / 256 overrides the tile-width heuristic
   int64_t gemm_splitk = 1;   // 1: split K over idle SMs when the tiles fill at most half of them
   int64_t push_sync = 1;     // how push-GEMM CTAs retire (GemmParams::push_sync); 1 measured == 0
-  int64_t gemm_cluster = 2;  // 2: pair CTAs in clusters and multicast the B tile; 1: off
 };
 
 Runtime& rt();

@@ -8,7 +8,7 @@
 // F.cross_entropy in examples/torch/gpt_train.py:37-43).  With a 50257-word vocabulary and 4096
 // rows that chain moves ~8 GB through HBM per step in ATen (an fp32 copy of the logits, an fp32
 // log-softmax, an fp32 gradient, a bf16 copy of it, plus two padded re-copies for the TMA
-// alignment of the following GEMMs): 3.4 ms of an 18.7 ms step (profiles/r01_final_launch_list_*).
+// alignment of the following GEMMs).
 // Here the logits are read once in their storage dtype for the forward (online max / sum-exp per
 // row, fp32 accumulation) and once for the backward, which writes the gradient straight into a
 // TMA-legal (row stride % 8 == 0) bf16 buffer that the two LM-head GEMMs consume without staging:

@@ -1,6 +1,6 @@
 // Runtime core of libedb.so: process state, symmetric heap, CUDA-IPC peer mapping, groups.
 //
-// Replaces (B200-native) what the reference gets from ProcessGroupNCCL + _expand_group
+// Replaces (natively on the GPU) what the reference gets from ProcessGroupNCCL + _expand_group
 // (easydist/torch/passes/sharding.py:95) and the DeviceMesh rank bookkeeping
 // (easydist/torch/device_mesh.py:129-150): instead of NCCL communicators we keep one
 // cudaMalloc'd slab per rank, mapped into every peer of the NVSwitch domain with CUDA IPC, and
@@ -238,7 +238,6 @@ int edb_set_option(const char* name, int64_t value) {
   else if (!strcmp(name, "copy_ctas_per_sm")) r.copy_ctas_per_sm = value;
   else if (!strcmp(name, "comm_ctas")) r.comm_ctas = value;
   else if (!strcmp(name, "spin_timeout_ms")) r.spin_timeout_ms = value;
-  else if (!strcmp(name, "gemm_cluster")) r.gemm_cluster = value;
   else if (!strcmp(name, "gemm_splitk")) r.gemm_splitk = value;
   else if (!strcmp(name, "gemm_force_bn")) r.gemm_force_bn = value;
   else if (!strcmp(name, "ll_max_bytes")) r.ll_max_bytes = value;
@@ -253,7 +252,6 @@ int edb_get_option(const char* name, int64_t* out) {
   else if (!strcmp(name, "copy_ctas_per_sm")) *out = r.copy_ctas_per_sm;
   else if (!strcmp(name, "comm_ctas")) *out = r.comm_ctas;
   else if (!strcmp(name, "spin_timeout_ms")) *out = r.spin_timeout_ms;
-  else if (!strcmp(name, "gemm_cluster")) *out = r.gemm_cluster;
   else if (!strcmp(name, "gemm_splitk")) *out = r.gemm_splitk;
   else if (!strcmp(name, "gemm_force_bn")) *out = r.gemm_force_bn;
   else if (!strcmp(name, "ll_max_bytes")) *out = r.ll_max_bytes;

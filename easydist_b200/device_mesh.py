@@ -4,7 +4,7 @@ Mirror of what the lowering needs from easydist/torch/device_mesh.py: `size(dim)
 `get_coordinate()`, the flat rank list of the sub-mesh along one dim through this rank's
 coordinate (sharding.py:725-730), and the 'spmd' alias binding of dims whose name contains
 "spmd" (device_mesh.py:115-121).  Unlike NDDeviceMesh it accepts size-1 dims, which is how the
-"1 x B200" configuration runs through the same compiled path (the reference does not compile at
+"1 x H100" configuration runs through the same compiled path (the reference does not compile at
 world size 1: api.py:117-118, device_mesh.py:39-41).
 """
 import numpy as np

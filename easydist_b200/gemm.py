@@ -3,7 +3,7 @@
 The sharded FX graph the reference executes calls ATen for every compute node
 (easydist/torch/compile_auto.py:752-756 runs the GraphModule op by op; the Linear layers are
 `aten.mm` / `aten.addmm`).  Here bf16 `aten.mm` / `aten.addmm` nodes are dispatched to the
-hand-written tcgen05 GEMM of libedb.so:
+hand-written wgmma GEMM of libedb.so:
 
   * all four operand layouts (row/column-major A and B) map to kernel variants, so Linear forward,
     dgrad and wgrad need no transposes;
@@ -242,7 +242,7 @@ def _count_unsupported(a, b):
 
 
 def mm(a, b, *, _side=0, _pf=None):
-    """aten.mm.default(a, b) with bf16 operands on the tcgen05 kernel.  `_side=1`: launched on the
+    """aten.mm.default(a, b) with bf16 operands on the wgmma kernel.  `_side=1`: launched on the
     side stream; some later `join` of the result (or of a view of it) must precede its first use.
     `_pf`: all-gather prefetch carried by this launch ({"group": ranks, "items": [(src_off,
     dst_off, bytes, dst_stride), ...]}, see edb_gemm_pf_bf16)."""

@@ -1,4 +1,4 @@
-"""Plan -> executable graph: the B200 replacement of the reference's lowering passes.
+"""Plan -> executable graph: the H100 replacement of the reference's lowering passes.
 
   sharding_transform(fx_module, opt_strategy, state_io_map)
         drop-in for easydist/torch/passes/sharding.py:852-979 (call site compile_auto.py:569):
@@ -13,9 +13,9 @@
         zero3), generalised from "the `_fused_adam` node" to any elementwise optimizer by working
         on the optimizer region of the graph (everything downstream of the final gradients).
   assign_static_buffers / dispatch_compute / propagate_local_meta
-        B200-specific finishing passes: symmetric-heap buffers fixed at compile time (so the
+        runtime-specific finishing passes: symmetric-heap buffers fixed at compile time (so the
         graph is CUDA-graph capturable with zero allocations in the comm path), bf16 `aten.mm` ->
-        tcgen05 GEMM dispatch.
+        wgmma GEMM dispatch.
 
 The emitted `call_function` targets are the callables of an `ops` namespace with the reference's
 names and signatures (default: easydist_b200.reshard -> libedb.so).
@@ -1235,7 +1235,7 @@ def fuse_gemm_epilogues(gm):
 
 
 def dispatch_compute(gm):
-    """Route bf16 `aten.mm` / `aten.addmm` nodes to the tcgen05 GEMM (sharded-op kernel dispatch)."""
+    """Route bf16 `aten.mm` / `aten.addmm` nodes to the wgmma GEMM (sharded-op kernel dispatch)."""
     import os
     from . import gemm, norm
     native_ln = os.environ.get("EDB_NATIVE_LN", "1") == "1"
@@ -1501,7 +1501,7 @@ def ensure_end_barrier(gm, ranks, ops=_default_ops):
 
 
 def fuse_collective_gemms(gm, io, rt, ranks, ops=_default_ops, my_index=None):
-    """Peephole fusion of reshard edges into the adjacent GEMM (B200 runtime only):
+    """Peephole fusion of reshard edges into the adjacent GEMM (libedb runtime only):
 
       all_gather(param shard) -> view -> t -> mm/addmm        ==>  ops.ag_mm   (AG + GEMM, one kernel)
       mm -> flatten -> reduce_scatter(avg, dim 0)              ==>  ops.mm_rs   (GEMM + RS, one kernel)
@@ -1702,7 +1702,7 @@ def fuse_collective_gemms(gm, io, rt, ranks, ops=_default_ops, my_index=None):
 
 def verify_epoch_protocol(gm, ops, n):
     """Static race check of a lowered graph against the contract of the epoch protocol (edb.h,
-    DESIGN.md §3.1) — the B200-native counterpart of the reference's debug-time `op_mem_checker`
+    DESIGN.md §3.1) — the libedb counterpart of the reference's debug-time `op_mem_checker`
     (an interval-tree ownership check per node, compile_auto.py:269-351), done once at compile time
     because here the hazards are decided by graph structure, not by run-time addresses:
 

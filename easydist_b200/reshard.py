@@ -554,7 +554,7 @@ def mm_rs_push(a, b, group, *, _buf, _lane=0):
 
 
 def mm_push(a, b, group, *, _buf):
-    """Epoch-mode push half of mm_rs: a @ b on the regular GEMM path (cta_group::2 pairs, split-K)
+    """Epoch-mode push half of mm_rs: a @ b on the regular GEMM path (split-K included)
     with every row block stored into its owner's receive slot over NVLink; no flags at all — the
     epoch barrier in front of `rs_finish(_epoch=1)` makes the slots complete.  _buf = (symmetric
     offset of the n receive slots,).  Returns an empty token for graph ordering."""

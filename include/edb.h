@@ -160,7 +160,7 @@ int edb_symm_guard(int gid, void* stream);
 
 /* ---- dense compute on the path (sharded-op kernel dispatch) ------------------------------- */
 
-/* C[M,N] (bf16, row-major, ldc) = A·B (+ bias) with fp32 accumulation on tcgen05 tensor cores.
+/* C[M,N] (bf16, row-major, ldc) = A·B (+ bias) with fp32 accumulation on Hopper (wgmma) tensor cores.
  *   a_kmajor: A is [M,K] row-major (lda = elements between rows)   else A is stored [K,M] (lda between k rows)
  *   b_kmajor: B is [N,K] row-major (i.e. C = A·Bᵀ, nn.Linear fwd)  else B is stored [K,N] (ldb between k rows)
  * Replaces the aten.mm.default nodes of the sharded graph (Linear fwd / dgrad / wgrad;
@@ -294,7 +294,7 @@ int edb_gemm_pf_bf16(void* C, const void* A, const void* B, const void* bias, in
                      void* stream);
 
 /* GEMM whose result is reduce-scattered over its rows, push half: C = A.B (operand layouts as
- * edb_gemm_bf16, incl. cta_group::2 pairs and split-K); row block [p*M/n, (p+1)*M/n) is stored
+ * edb_gemm_bf16, incl. split-K); row block [p*M/n, (p+1)*M/n) is stored
  * straight into member p's receive slot [me] at symmetric `recv_off` (n slots of (M/n)*N*2 bytes
  * on every member, dedicated to this GEMM) over NVLink, next member's rows first, own rows last.
  * No flags: after the next edb_epoch_barrier every slot of every member is complete, and
@@ -368,7 +368,7 @@ int edb_sgd_momentum(int n, void* const* params, const void* const* grads, void*
 /* ---- options / introspection --------------------------------------------------------------- */
 
 /* integer options: "allreduce_oneshot_bytes", "copy_ctas_per_sm", "comm_ctas", "spin_timeout_ms",
- * "ll_max_bytes", "gemm_cluster", "gemm_force_bn", "gemm_splitk" */
+ * "ll_max_bytes", "gemm_force_bn", "gemm_splitk" */
 int edb_set_option(const char* name, int64_t value);
 int edb_get_option(const char* name, int64_t* value_out);
 /* number of kernels this library has launched since load (all entry points) */

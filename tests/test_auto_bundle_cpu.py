@@ -36,8 +36,9 @@ def train_step(input, model, opt):
     return out
 
 
-def run_bundle(rank, world, mesh_shape, ops, native, device):
-    """Shared by the CPU test and the GPU worker.  Returns (ok, message, comm histogram)."""
+def run_bundle(rank, world, mesh_shape, ops, native, device, planner="GREEDY"):
+    """Shared by the CPU test and the GPU worker.  Returns (ok, message, comm histogram).
+    `planner`: the reshard planner the lowering uses (the solved plan does not depend on it)."""
     import numpy as np
     from easydist_b200 import api
     from easydist_b200.device_mesh import set_device_mesh
@@ -53,7 +54,8 @@ def run_bundle(rank, world, mesh_shape, ops, native, device):
     ropt = torch.optim.SGD(ref.parameters(), lr=0.1, momentum=0.9, foreach=True)
     g = torch.Generator().manual_seed(7)
     batches = [torch.randn(16, 64, generator=g).to(device) for _ in range(3)]
-    compiled = api.compile_from_bundle(bundle, (batches[0], model, opt), {}, ops=ops, native=native)
+    compiled = api.compile_from_bundle(bundle, (batches[0], model, opt), {}, ops=ops, native=native,
+                                       planner=planner)
     ok, msg = True, ""
     for b in batches:
         out = compiled(b, model, opt)
@@ -63,7 +65,7 @@ def run_bundle(rank, world, mesh_shape, ops, native, device):
     return ok, msg, compiled.info["comm_nodes"]
 
 
-def _worker(rank, world, mesh_shape, port, q, bucket="0"):
+def _worker(rank, world, mesh_shape, port, q, bucket="0", planner="GREEDY"):
     os.environ["OMP_NUM_THREADS"] = "1"
     os.environ["EDB_BUCKET_COMM"] = bucket
     torch.set_num_threads(1)
@@ -72,11 +74,31 @@ def _worker(rank, world, mesh_shape, port, q, bucket="0"):
     import numpy as np
     from tests import gloo_ops
     gloo_ops.init_groups(np.arange(world).reshape(mesh_shape))
-    ok, msg, hist = run_bundle(rank, world, mesh_shape, gloo_ops, False, "cpu")
+    ok, msg, hist = run_bundle(rank, world, mesh_shape, gloo_ops, False, "cpu", planner=planner)
     if rank == 0:
         q.put((ok, msg, hist))
     dist.barrier()
     dist.destroy_process_group()
+
+
+@pytest.mark.parametrize("planner,want", [
+    # the reference's own lowering of this plan with that planner (tests/ref/auto_worker.py with
+    # EDB_TEST_MESH=2x2 EDB_PLANNER=<planner> EDB_SAMEPLAN=1, `hist_ref_same_plan`); P2P's
+    # histogram equals GREEDY's on this plan, REPLICATE gathers instead of all-to-all
+    ("REPLICATE", {"all_gather_start": 45, "scatter_wrapper": 27, "reduce_scatter_start": 1,
+                   "all_reduce_start": 5, "all_to_all_start": 0}),
+    ("P2P", {"all_gather_start": 37, "scatter_wrapper": 19, "reduce_scatter_start": 1,
+             "all_reduce_start": 5, "all_to_all_start": 2}),
+])
+def test_recorded_reference_plan_lowers_like_the_reference_with_other_planners(planner, want):
+    """The drop-in lowering with the REPLICATE and P2P reshard planners on a 2x2 mesh: the plan
+    the reference solved, lowered by this backend, matches vanilla PyTorch and has the same
+    communication structure as the reference's lowering of that plan."""
+    ok, msg, hist = run_world(_worker, 4, lambda r, port, q: (r, 4, (2, 2), port, q, "0", planner),
+                              timeout=240)
+    assert ok, msg
+    for k, v in want.items():
+        assert hist.get(k, 0) == v, (k, hist)
 
 
 @pytest.mark.parametrize("mesh_shape", [(2,), (2, 2)])
@@ -243,6 +265,37 @@ def test_config1_gpt_plan_from_the_reference_solver_matches_vanilla():
         assert hist.get(k, 0) == v, (k, hist)
 
 
+def _gpt_test_worker(rank, world, port, q):
+    os.environ["OMP_NUM_THREADS"] = "1"
+    torch.set_num_threads(1)
+    dist.init_process_group("gloo", init_method=f"tcp://127.0.0.1:{port}", rank=rank,
+                            world_size=world)
+    import numpy as np
+    from tests import gloo_ops
+    gloo_ops.init_groups(np.arange(world).reshape((world,)))
+    ok, msg, hist = run_c1_bundle(rank, world, gloo_ops, False, "cpu", steps=2,
+                                  bundle_file=os.path.join(GOLDEN, "auto_gpt_test_mesh2.json.gz"),
+                                  gpt=(2, 64, 4), batch=4, seq=32)
+    if rank == 0:
+        q.put((ok, msg, hist))
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+def test_reference_test_gpt_plan_lowers_like_the_reference():
+    """The reference's own GPT test model (depth 2, dim 64, 4 heads; batch 4 x 32) with the plan its
+    solver produced at mesh (2,) (recorded by tests/ref/auto_worker.py with EDB_MODEL=gpt
+    EDB_SAMEPLAN=1): this backend's lowering matches vanilla PyTorch in outputs, every parameter and
+    every momentum buffer, and has the communication structure of the reference's lowering of the
+    same plan (`hist_ref_same_plan` of that run)."""
+    ok, msg, hist = run_world(_gpt_test_worker, 2, lambda r, port, q: (r, 2, port, q), timeout=300)
+    assert ok, msg
+    want = {"all_gather_start": 215, "scatter_wrapper": 99, "reduce_scatter_start": 14,
+            "all_reduce_start": 9, "all_to_all_start": 8}
+    for k, v in want.items():
+        assert hist.get(k, 0) == v, (k, hist)
+
+
 def test_config1_optimizer_runs_on_shards_when_localized():
     """lowering.localize_foreach on the same plan: the optimizer's foreach ops run on the shards
     (the reference gathers every parameter / gradient / state in front of each of them and scatters
@@ -317,7 +370,7 @@ def test_config1_plans_for_larger_meshes_lower_to_the_recorded_structure(tag, me
      {"all_gather_start": 2569, "scatter_wrapper": 1177, "reduce_scatter_start": 72,
       "all_reduce_start": 97, "all_to_all_start": 144}),
     # ... and at world 8 (capture-only recording: no reference-lowering histogram to compare with;
-    # executed against vanilla with tools/validate_bundle.py, profiles/r02_auto_gpt2medium_plan_*)
+    # executed against vanilla with tools/validate_bundle.py)
     ("gpt2medium_s128_mesh8", (24, 1024, 16), 8, 3, 8, 128, None),
 ])
 def test_gpt2_small_and_medium_size_plans_lower_to_the_recorded_structure_and_pass_the_static_check(

@@ -1,6 +1,6 @@
-"""Single-GPU parity tests (B200): every call goes through the C-ABI (ctypes -> libedb.so).
+"""Single-GPU parity tests (H100): every call goes through the C-ABI (ctypes -> libedb.so).
   * local reshard ops and n=1 collectives vs the oracle (bit-exact)
-  * tcgen05 GEMM vs a plain PyTorch fp32 reference (floating point: tolerance stated below)
+  * wgmma GEMM vs a plain PyTorch fp32 reference (floating point: tolerance stated below)
 """
 import numpy as np
 import pytest

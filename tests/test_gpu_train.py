@@ -1,4 +1,4 @@
-"""End-to-end train step through the compiled path on one B200 vs the oracle (CPU fp32
+"""End-to-end train step through the compiled path on one H100 vs the oracle (CPU fp32
 restatement of the same step).  bf16 GPU vs fp32 CPU: the loss trajectory must agree within 3e-2
 relative (bf16 keeps 8 mantissa bits; the reference's own comparator uses rtol 1e-4 for fp32,
 tests/test_torch/test_spmd.py:67, which is what the fp32 case below holds itself to)."""

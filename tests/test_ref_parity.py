@@ -1,7 +1,11 @@
-"""Reference-in-the-loop parity (CPU container only: needs /root/reference).  The unmodified
+"""Reference-in-the-loop parity (needs the original easydist sources, EASYDIST_REFERENCE).  The unmodified
 reference traces, annotates and solves; its lowering (A) and the drop-in
 easydist_b200.lowering.sharding_transform (B) are run on the same plan and inputs over gloo and
-compared with each other and with vanilla PyTorch — tests/ref/auto_worker.py."""
+compared with each other and with vanilla PyTorch — tests/ref/auto_worker.py.  Every case of
+test_dropin_lowering_equals_reference_lowering has a recorded counterpart in
+tests/test_auto_bundle_cpu.py (the reference's plan + its lowering's communication histogram,
+replayed without the reference); the plugin-hook tests drive the reference's own decorator and
+have none."""
 import os
 import sys
 
@@ -9,6 +13,7 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from oracle.refcompat import REFERENCE_ROOT  # noqa: E402
 from tests._procs import run_torchrun  # noqa: E402
 pytestmark = pytest.mark.refonly
 
@@ -19,8 +24,8 @@ pytestmark = pytest.mark.refonly
     ("2", 2, "GREEDY", "gpt"),   # the reference's GPT test model: views, expand, bmm
 ])
 def test_dropin_lowering_equals_reference_lowering(mesh, nproc, planner, model):
-    if not os.path.isdir("/root/reference/easydist"):
-        pytest.skip("reference not present (GPU box)")
+    if not os.path.isdir(os.path.join(REFERENCE_ROOT, "easydist")):
+        pytest.skip("original easydist sources not present (set EASYDIST_REFERENCE)")
     env = dict(os.environ, EDB_TEST_MESH=mesh, OMP_NUM_THREADS="1", EDB_PLANNER=planner,
                EDB_MODEL=model, EDB_SAMEPLAN="1")
     rc, out, err = run_torchrun(os.path.join(ROOT, "tests", "ref", "auto_worker.py"), nproc, env,
@@ -42,8 +47,8 @@ def test_plugin_hook_through_the_reference_decorator(mode):
     the same call; "b200_auto" = Hook C: the reference's tracing + annotation + ILP produce the plan,
     this backend lowers AND executes it (its own EDCompiledFunc, no per-step distribute_tensor) —
     tests/ref/plugin_worker.py."""
-    if not os.path.isdir("/root/reference/easydist"):
-        pytest.skip("reference not present (GPU box)")
+    if not os.path.isdir(os.path.join(REFERENCE_ROOT, "easydist")):
+        pytest.skip("original easydist sources not present (set EASYDIST_REFERENCE)")
     env = dict(os.environ, OMP_NUM_THREADS="1", EDB_PLUGIN_MODE=mode)
     if mode == "auto+localize":
         # Hook B with the optimizer localized: the REFERENCE's executor runs the rewritten graph

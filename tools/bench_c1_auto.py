@@ -34,7 +34,7 @@ def main():
     ap.add_argument("--gpt", default="", help="depth,dim,heads,batch,seq of the bundle's model")
     ap.add_argument("--dtype", default="fp32", choices=["fp32", "bf16"],
                     help="bf16: parameters and inputs in bf16 (the plan is dtype independent; the "
-                         "Linear layers then run on the native tcgen05 GEMM)")
+                         "Linear layers then run on the native wgmma GEMM)")
     run(ap.parse_args())
 
 

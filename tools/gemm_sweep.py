@@ -1,4 +1,4 @@
-"""Tile-shape / cluster sweep of the tcgen05 GEMM vs cuBLAS (tuning aid)."""
+"""Tile-width sweep of the wgmma GEMM vs cuBLAS (tuning aid)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -21,10 +21,9 @@ for (M,N,K) in shapes:
     t_ref = timeit(lambda: torch.mm(a, w.t()))
     t_ref_warm = timeit(lambda: torch.mm(a, w.t()), do_flush=False)
     row = [f"cublas {t_ref*1e3:7.1f}us {fl/t_ref/1e9:5.0f}TF (warm {t_ref_warm*1e3:.1f}us)"]
-    for cl in (1,2):
-        for bn in (128,256):
-            rt.set_option("gemm_cluster", cl); rt.set_option("gemm_force_bn", bn)
-            t = timeit(lambda: gemm.mm(a, w.t()))
-            tw = timeit(lambda: gemm.mm(a, w.t()), do_flush=False)
-            row.append(f"cl{cl}bn{bn} {t*1e3:7.1f}us {fl/t/1e9:5.0f}TF (warm {tw*1e3:.1f})")
+    for bn in (128,256):
+        rt.set_option("gemm_force_bn", bn)
+        t = timeit(lambda: gemm.mm(a, w.t()))
+        tw = timeit(lambda: gemm.mm(a, w.t()), do_flush=False)
+        row.append(f"bn{bn} {t*1e3:7.1f}us {fl/t/1e9:5.0f}TF (warm {tw*1e3:.1f})")
     print(f"{(M,N,K)}: " + " | ".join(row), flush=True)
