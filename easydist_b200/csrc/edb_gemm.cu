@@ -1296,8 +1296,10 @@ static int check_operands(const void* A, const void* B, const void* C, const voi
   return EDB_OK;
 }
 
-// fp32 workspace of split-K GEMMs: one slab per (device, stream) pair, allocated on first use
-// (outside any stream capture: the compiled step always runs eagerly once before it is captured).
+// fp32 workspace of split-K GEMMs: one slab per (device, stream) pair, allocated on first use and
+// never freed, so a CUDA graph that captured a slab's address may replay at any later time.  The
+// first use may come while the stream is being captured: torch.cuda.graph captures on a stream of its
+// own, not on the one its eager warm-up ran on.
 constexpr size_t kSplitKBytes = (size_t)64 << 20;
 struct SplitKSlab {
   int device;
@@ -1313,13 +1315,17 @@ static float* splitk_workspace(cudaStream_t st) {
   for (int i = 0; i < g_splitk_n; ++i)
     if (g_splitk[i].device == dev && g_splitk[i].stream == st) return g_splitk[i].ptr;
   if (g_splitk_n == 16) return nullptr;
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(st, &cs) != cudaSuccess || cs != cudaStreamCaptureStatusNone) {
+  // cudaMalloc enqueues nothing on `st`, so it is safe during a capture; a capture begun in the
+  // (default) global mode forbids it unless this thread switches to relaxed mode for the call
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  if (cudaThreadExchangeStreamCaptureMode(&mode) != cudaSuccess) {
     cudaGetLastError();
-    return nullptr;  // cannot allocate while capturing: this launch runs unsplit
+    return nullptr;
   }
   float* ptr = nullptr;
-  if (cudaMalloc(&ptr, kSplitKBytes) != cudaSuccess) {
+  const cudaError_t err = cudaMalloc(&ptr, kSplitKBytes);
+  cudaThreadExchangeStreamCaptureMode(&mode);  // restore the caller's mode
+  if (err != cudaSuccess) {
     cudaGetLastError();
     return nullptr;
   }

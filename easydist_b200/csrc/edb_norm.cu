@@ -183,7 +183,9 @@ __global__ void __launch_bounds__(kLnWarps * 32, (NV <= 4 ? 2 : 1))
         LnT<T>::unpack(LnT<T>::pack(o), r1);  // round to T first, like the separate kernels do
         LnT<T>::unpack(ac[i], av);
 #pragma unroll
-        for (int e = 0; e < EPV; ++e) o[e] = r1[e] + av[e];
+        // __fadd_rn: for T = float the rounding to T is a no-op, and a plain + would be contracted
+        // with the product above into one FMA (one rounding instead of ATen's two)
+        for (int e = 0; e < EPV; ++e) o[e] = __fadd_rn(r1[e], av[e]);
       }
       dr[i * 32 + lane] = LnT<T>::pack(o);
     }
