@@ -105,7 +105,15 @@ SIGNATURES = {
                                        c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
                                        c_int, c_void_p]),
     "edb_layer_norm_bwd_workspace": (c_int, [c_int64, POINTER(c_size_t)]),
-    "edb_colsum": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int, c_void_p]),
+    "edb_rms_norm_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_float,
+                                 c_int, c_int, c_void_p]),
+    "edb_rms_norm_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                 c_void_p, c_int64, c_int64, c_int, c_int, c_void_p]),
+    "edb_rms_norm_bwd_workspace": (c_int, [c_int64, POINTER(c_size_t)]),
+    "edb_swiglu_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
+    "edb_swiglu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
+                               c_void_p]),
+    "edb_colsum": (c_int,[c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int, c_void_p]),
     "edb_colsum_workspace": (c_int, [c_int64, POINTER(c_size_t)]),
     "edb_cross_entropy_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
                                       c_void_p, c_int64, c_int64, c_int64, c_int, c_int, c_void_p]),

@@ -997,6 +997,316 @@ def fuse_cross_entropy(gm):
     return n
 
 
+def _call(nd, *targets):
+    return isinstance(nd, Node) and nd.op == "call_function" and nd.target in targets
+
+
+def _mul_other(mul, x):
+    """The operand of the binary aten.mul.Tensor node `mul` that is not `x` (None if x is not one)."""
+    if not _call(mul, aten.mul.Tensor) or len(mul.args) != 2 or mul.kwargs:
+        return None
+    a, b = mul.args
+    return b if a is x else (a if b is x else None)
+
+
+def _only_user(nd):
+    return next(iter(nd.users)) if len(nd.users) == 1 else None
+
+
+def _match_rms_chain(r):
+    """The decomposed RMSNorm around rsqrt node `r` (workloads.RMSNorm and its autograd backward,
+    with or without the fp32 round trip) -> dict of its parts, or None.  Every intermediate must have
+    exactly the users the chain gives it."""
+    def val(nd):
+        return nd.meta.get("val") if isinstance(nd, Node) else None
+
+    def f32_copy_of(nd):
+        if _call(nd, aten._to_copy.default) and len(nd.args) == 1 \
+                and nd.kwargs.get("dtype") == torch.float32 \
+                and set(nd.kwargs) <= {"dtype", "layout", "device"}:
+            return nd.args[0]
+        return None
+
+    def cast_to(nd, dtype):
+        """nd == _to_copy(src, dtype) -> src."""
+        if _call(nd, aten._to_copy.default) and len(nd.args) == 1 and nd.kwargs.get("dtype") == dtype \
+                and set(nd.kwargs) <= {"dtype", "layout", "device"}:
+            return nd.args[0]
+        return None
+
+    add = r.args[0] if len(r.args) == 1 and not r.kwargs else None
+    if not (_call(add, aten.add.Tensor) and len(add.users) == 1 and len(add.args) == 2
+            and isinstance(add.args[1], (int, float)) and not add.kwargs):
+        return None
+    mean, eps = add.args
+    if not (_call(mean, aten.mean.dim) and len(mean.users) == 1 and len(mean.args) == 3
+            and mean.args[2] is True and not mean.kwargs):
+        return None
+    pw2 = mean.args[0]
+    if not (_call(pw2, aten.pow.Tensor_Scalar) and pw2.args[1] == 2 and len(pw2.users) == 1):
+        return None
+    xa = pw2.args[0]
+    x = f32_copy_of(xa)
+    cast = x is not None
+    if not cast:
+        x = xa
+    xv = val(x)
+    if not isinstance(xv, torch.Tensor) or xv.dim() < 2 or (xv.dtype == torch.float32) == cast:
+        return None
+    nd_, H = xv.dim(), int(xv.shape[-1])
+    last = [[-1], [nd_ - 1]]
+    if list(mean.args[1]) not in last:
+        return None
+
+    def is_x(nd):  # x itself or (bf16 model) one of its fp32 copies
+        return nd is x if not cast else f32_copy_of(nd) is x
+
+    if len(r.users) != 3:
+        return None
+    n32 = p1 = pw3 = None
+    for u in r.users:
+        if _call(u, aten.pow.Tensor_Scalar) and u.args[0] is r and u.args[1] == 3:
+            pw3 = u
+        elif _mul_other(u, r) is not None and is_x(_mul_other(u, r)):
+            n32 = u
+        elif _mul_other(u, r) is not None:
+            p1 = u
+    if n32 is None or p1 is None or pw3 is None or len(pw3.users) != 1:
+        return None
+    nb = n32
+    if cast:
+        nb = _only_user(n32)
+        if cast_to(nb, xv.dtype) is not n32:
+            return None
+    if len(nb.users) != 2:
+        return None
+    def shaped(nd, shape):  # graph transforms insert nodes without meta: unknown shapes pass
+        v = val(nd)
+        return isinstance(nd, Node) and (v is None or tuple(v.shape) == tuple(shape))
+
+    # the forward's mul(normed, w) and the backward's mul(dy, normed), whose only reader is the dw sum
+    y = dwm = w_f = dy = None
+    for u in nb.users:
+        o = _mul_other(u, nb)
+        if _call(_only_user(u), aten.sum.dim_IntList) and shaped(o, xv.shape):
+            dwm, dy = u, o
+        elif shaped(o, (H,)):
+            y, w_f = u, o
+    if y is None or dwm is None:
+        return None
+    sm = _only_user(dwm)
+    if not (_call(sm, aten.sum.dim_IntList) and len(sm.args) == 3 and sm.args[2] is True
+            and sorted(d % nd_ for d in sm.args[1]) == list(range(nd_ - 1)) and not sm.kwargs):
+        return None
+    # backward: g = dy*w (-> fp32), p1 = g*rstd, gx = g*x
+    g32 = _mul_other(p1, r)
+    g = f32_copy_of(g32) if cast else g32
+    if g is None or len(g32.users) != 2 or (cast and len(g.users) != 1):
+        return None
+    w_b = _mul_other(g, dy)
+    if w_b is None or not shaped(w_b, (H,)):
+        return None
+    gx = next(u for u in g32.users if u is not p1)
+    if _mul_other(gx, g32) is None or not is_x(_mul_other(gx, g32)) or len(gx.users) != 1:
+        return None
+    s = _only_user(gx)
+    if not (_call(s, aten.sum.dim_IntList) and len(s.args) == 3 and list(s.args[1]) in last
+            and s.args[2] is True and len(s.users) == 1):
+        return None
+    ms = _only_user(s)
+    if not (_call(ms, aten.mul.Scalar) and ms.args == (s, -0.5) and len(ms.users) == 1):
+        return None
+    m5 = _only_user(ms)
+    if _mul_other(m5, ms) is not pw3 or _only_user(pw3) is not m5 or len(m5.users) != 1:
+        return None
+    ex = _only_user(m5)
+    if not (_call(ex, aten.expand.default) and list(ex.args[1]) == list(xv.shape)
+            and len(ex.users) == 1):
+        return None
+    dv = _only_user(ex)
+    if not (_call(dv, aten.div.Scalar) and dv.args[1] == H and len(dv.users) == 1):
+        return None
+    p2 = _only_user(dv)
+    q = _mul_other(p2, dv)
+    if not (_call(q, aten.mul.Scalar) and q.args[1] == 2.0 and len(q.users) == 1):
+        return None
+    pw1 = q.args[0]
+    if not (_call(pw1, aten.pow.Tensor_Scalar) and pw1.args[1] == 1.0 and len(pw1.users) == 1
+            and is_x(pw1.args[0])):
+        return None
+    pieces = []
+    for p in (p1, p2):
+        if len(p.users) != 1:
+            return None
+        pc = _only_user(p) if cast else p
+        if cast and cast_to(pc, xv.dtype) is not p:
+            return None
+        if len(pc.users) != 1:
+            return None
+        pieces.append(pc)
+    p1c, p2c = pieces
+    u1, u2 = _only_user(p1c), _only_user(p2c)
+    run = None
+    if u1 is u2 and _call(u1, aten.add.Tensor) and len(u1.args) == 2 \
+            and set(u1.args) == {p1c, p2c} and not u1.kwargs:
+        dx = u1
+    elif _call(u1, aten.add.Tensor) and len(u1.args) == 2 and not u1.kwargs and p1c in u1.args \
+            and _only_user(u1) is u2 and _call(u2, aten.add.Tensor) and len(u2.args) == 2 \
+            and not u2.kwargs and set(u2.args) == {u1, p2c}:
+        run = u1.args[1] if u1.args[0] is p1c else u1.args[0]
+        rv = val(run)
+        if not isinstance(run, Node) or run in (p1c, p2c) or not isinstance(rv, torch.Tensor) \
+                or tuple(rv.shape) != tuple(xv.shape) or rv.dtype != xv.dtype:
+            return None
+        dx = u2
+    else:
+        return None
+    chain = [y, n32, r, add, mean, pw2, dwm, sm, g32, p1, gx, s, ms, pw3, m5, ex, dv, q, pw1, p2, dx]
+    if cast:
+        chain += [nb, g, p1c, p2c]
+    if run is not None:
+        chain.append(u1)
+    copies = list({xa, _mul_other(n32, r), _mul_other(gx, g32), pw1.args[0]}) if cast else []
+    return dict(x=x, w_f=w_f, w_b=w_b, dy=dy, eps=eps, y=y, r=r, sm=sm, dx=dx, run=run,
+                chain=chain, x_copies=copies)
+
+
+def fuse_rms_norm(gm):
+    """Rewrite RMSNorm onto edb_rms.cu (norm.rms_norm_fwd / rms_norm_bwd):
+
+    (a) the decomposed chain `(x.float() * rsqrt(x.float().pow(2).mean(-1, keepdim=True) + eps))
+        .to(x.dtype) * w` (workloads.RMSNorm; the fp32 casts are absent in an fp32 model) together
+        with its autograd backward, found from the forward's saved rstd / normed / fp32-x nodes; the
+        `add`s of the two dx pieces onto the running gradient of x become `_add`;
+    (b) aten._fused_rms_norm / _fused_rms_norm_backward nodes (F.rms_norm, nn.RMSNorm on CUDA),
+        retargeted to norm.fused_rms_norm(_backward), with a following add(dx, g) folded into `_add`.
+    Chains with any extra reader of an intermediate are left alone.  Returns (forward, backward)
+    counts."""
+    import operator
+    from . import norm
+    graph = gm.graph
+    n_fwd = n_bwd = 0
+    for r in [nd for nd in graph.nodes if _call(nd, aten.rsqrt.default)]:
+        m = _match_rms_chain(r)
+        if m is None:
+            continue
+        order = {nd: i for i, nd in enumerate(graph.nodes)}
+        outs = list(m["sm"].users) + list(m["dx"].users)
+        at = min(outs, key=lambda u: order[u]) if outs else m["dx"]
+        ins = [m["dy"], m["x"], m["w_b"]] + ([m["run"]] if m["run"] is not None else [])
+        if any(order[i] >= order[at] for i in ins) or order[m["y"]] >= order[at]:
+            continue
+        with graph.inserting_before(m["y"]):
+            f = graph.call_function(norm.rms_norm_fwd, (m["x"], m["w_f"], m["eps"],
+                                                        norm.RMS_CAST_THEN_SCALE))
+            y2 = graph.call_function(operator.getitem, (f, 0))
+            rs2 = graph.call_function(operator.getitem, (f, 1))
+        y2.meta, rs2.meta = dict(m["y"].meta), dict(m["r"].meta)
+        m["y"].replace_all_uses_with(y2)
+        with graph.inserting_before(at):
+            kw = {"_add": m["run"]} if m["run"] is not None else {}
+            b = graph.call_function(norm.rms_norm_bwd, (m["dy"], m["x"], rs2, m["w_b"],
+                                                        norm.RMS_CAST_THEN_SCALE, [True, True]), kw)
+            dx2 = graph.call_function(operator.getitem, (b, 0))
+            dw2 = graph.call_function(operator.getitem, (b, 1))
+            dwv = graph.call_function(aten.view.default, (dw2, list(m["sm"].meta["val"].shape)))
+        dx2.meta, dwv.meta = dict(m["dx"].meta), dict(m["sm"].meta)
+        m["dx"].replace_all_uses_with(dx2)
+        m["sm"].replace_all_uses_with(dwv)
+        # erase exactly the replaced chain, readers first
+        for d in sorted(m["chain"], key=lambda nd: -order[nd]):
+            assert not d.users, (d, list(d.users))
+            graph.erase_node(d)
+        for c in m["x_copies"]:
+            if not c.users:
+                graph.erase_node(c)
+        n_fwd += 1
+        n_bwd += 1
+    # (b) the fused ATen ops
+    for nd in list(graph.nodes):
+        if _call(nd, aten._fused_rms_norm.default):
+            nd.target = norm.fused_rms_norm
+            n_fwd += 1
+        elif _call(nd, aten._fused_rms_norm_backward.default):
+            nd.target = norm.fused_rms_norm_backward
+            n_bwd += 1
+    order = {nd: i for i, nd in enumerate(graph.nodes)}
+    for nd in list(graph.nodes):
+        if not _call(nd, aten.add.Tensor) or len(nd.args) != 2 or nd.kwargs:
+            continue
+        for gi, oi in ((0, 1), (1, 0)):
+            g, other = nd.args[gi], nd.args[oi]
+            if not (_call(g, operator.getitem) and g.args[1] == 0 and len(g.users) == 1
+                    and isinstance(other, Node)):
+                continue
+            bw = g.args[0]
+            if not (_call(bw, norm.fused_rms_norm_backward) and "_add" not in bw.kwargs):
+                continue
+            gv, ov = g.meta.get("val"), other.meta.get("val")
+            if gv is None or ov is None or tuple(gv.shape) != tuple(ov.shape) \
+                    or gv.dtype != ov.dtype or order[other] > order[bw]:
+                continue
+            bw.kwargs = dict(bw.kwargs, _add=other)
+            nd.replace_all_uses_with(g)
+            graph.erase_node(nd)
+            break
+    if n_fwd or n_bwd:
+        graph.lint()
+        gm.recompile()
+    return n_fwd, n_bwd
+
+
+def fuse_swiglu(gm):
+    """`mul(silu(a), b)` and its backward `mul(dy, silu(a))`, `mul(dy, b)`, `silu_backward(., a)`
+    ==> act.swiglu_fwd(a, b) / act.swiglu_bwd(dy, a, b) (edb_rms.cu).  The silu node is erased: no
+    [tokens, ffn] tensor besides a and b stays alive from forward to backward.  Only a silu with
+    exactly those two readers is rewritten.  Returns (forward, backward) counts."""
+    import operator
+    from . import act
+    graph = gm.graph
+    n = 0
+    for s in [nd for nd in graph.nodes if _call(nd, aten.silu.default)]:
+        if len(s.args) != 1 or s.kwargs or len(s.users) != 2:
+            continue
+        a = s.args[0]
+        u = list(s.users)
+        found = None
+        for f, m1 in ((u[0], u[1]), (u[1], u[0])):
+            b, dy = _mul_other(f, s), _mul_other(m1, s)
+            if b is None or dy is None or b is s or dy is s:
+                continue
+            for m2 in b.users:
+                sb = _only_user(m2) if _mul_other(m2, b) is dy else None
+                if _call(sb, aten.silu_backward.default) and sb.args == (m2, a) and not sb.kwargs:
+                    found = (f, m1, m2, sb, b, dy)
+                    break
+            if found:
+                break
+        if found is None:
+            continue
+        f, m1, m2, sb, b, dy = found
+        order = {nd: i for i, nd in enumerate(graph.nodes)}
+        with graph.inserting_before(f):
+            out = graph.call_function(act.swiglu_fwd, (a, b))
+        out.meta = dict(f.meta)
+        f.replace_all_uses_with(out)
+        with graph.inserting_before(min((m1, m2), key=lambda nd: order[nd])):
+            bw = graph.call_function(act.swiglu_bwd, (dy, a, b))
+            dgate = graph.call_function(operator.getitem, (bw, 0))
+            dup = graph.call_function(operator.getitem, (bw, 1))
+        dgate.meta, dup.meta = dict(sb.meta), dict(m1.meta)
+        sb.replace_all_uses_with(dgate)
+        m1.replace_all_uses_with(dup)
+        for d in (sb, m2, m1, f, s):
+            assert not d.users, (d, list(d.users))
+            graph.erase_node(d)
+        n += 1
+    if n:
+        graph.lint()
+        gm.recompile()
+    return n, n
+
+
 def fuse_optimizer_updates(gm):
     """The re-inplaced update of torch.optim.SGD(momentum, foreach=True),
         _foreach_mul_(bufs, mu); _foreach_add_(bufs, grads[, alpha=a]); _foreach_add_(params, bufs, alpha=-lr)
@@ -1234,16 +1544,23 @@ def fuse_gemm_epilogues(gm):
     return n
 
 
-def dispatch_compute(gm):
-    """Route bf16 `aten.mm` / `aten.addmm` nodes to the wgmma GEMM (sharded-op kernel dispatch)."""
+def dispatch_compute(gm, counts=None):
+    """Route bf16 `aten.mm` / `aten.addmm` nodes to the wgmma GEMM (sharded-op kernel dispatch).
+    `counts` (a dict), when given, receives the (forward, backward) counts of the RMSNorm and SwiGLU
+    rewrites as "rms_norm" and "swiglu"."""
     import os
     from . import gemm, norm
     native_ln = os.environ.get("EDB_NATIVE_LN", "1") == "1"
+    counts = {} if counts is None else counts
     n = 0
     if os.environ.get("EDB_NATIVE_CE", "1") == "1":
         n += fuse_cross_entropy(gm)
     if os.environ.get("EDB_NATIVE_OPT", "1") == "1":
         n += fuse_optimizer_updates(gm)
+    # before the sum.dim_IntList retargeting below, which would otherwise claim the dw sums
+    counts["rms_norm"] = fuse_rms_norm(gm) if os.environ.get("EDB_NATIVE_RMS", "1") == "1" else (0, 0)
+    counts["swiglu"] = fuse_swiglu(gm) if os.environ.get("EDB_NATIVE_SWIGLU", "1") == "1" else (0, 0)
+    n += sum(counts["rms_norm"]) + sum(counts["swiglu"])
     for node in gm.graph.nodes:
         if node.op != "call_function":
             continue

@@ -330,6 +330,35 @@ int edb_layer_norm_bwd_add(void* dx, void* dw, void* db, const void* dy, const v
                            void* workspace, int64_t rows, int64_t H, int dtype, void* stream);
 int edb_layer_norm_bwd_workspace(int64_t H, size_t* bytes_out);
 
+/* RMSNorm over the last dimension — the decomposed Llama chain (pow, mean, add eps, rsqrt, mul, mul
+ * weight, with its ~17-op backward) and aten._fused_rms_norm(_backward) nodes of the sharded graph.
+ * x, y, dy, dx, add_in: [rows, H] contiguous; w, dw: [H]; all bf16 or f32 (`dtype`), 16-byte
+ * aligned; rstd: [rows] f32.  Forward: rstd = rsqrt(mean(x^2) + eps) in fp32 and
+ *   mode EDB_RMS_CAST_THEN_SCALE: y = T(T(x*rstd)*w)   (x.float() * rsqrt(...)).to(T) * w
+ *   mode EDB_RMS_FUSED:           y = T(x*rstd*w)      aten._fused_rms_norm
+ * Backward, in fp32 with n = x*rstd and g = dy*w (rounded to T in EDB_RMS_CAST_THEN_SCALE, as the
+ * chain's mul(dy, w) is): dx = T(add_in + rstd*(g - n*mean(g*n))), one rounding (no add_in when
+ * NULL); dw = T(sum over rows of dy*n^) with n^ = T(n) (CAST_THEN_SCALE) or n (FUSED), partials
+ * summed in a fixed order (deterministic); dw may be NULL.  Supported H: multiples of 8 (bf16) / 4
+ * (f32) up to 16384, else EDB_E_UNSUPPORTED.  `workspace`: edb_rms_norm_bwd_workspace(H) bytes. */
+#define EDB_RMS_CAST_THEN_SCALE 0
+#define EDB_RMS_FUSED 1
+int edb_rms_norm_fwd(void* y, void* rstd, const void* x, const void* w, int64_t rows, int64_t H,
+                     float eps, int mode, int dtype, void* stream);
+int edb_rms_norm_bwd(void* dx, void* dw, const void* dy, const void* x, const void* rstd,
+                     const void* w, const void* add_in, void* workspace, int64_t rows, int64_t H,
+                     int mode, int dtype, void* stream);
+int edb_rms_norm_bwd_workspace(int64_t H, size_t* bytes_out);
+
+/* SwiGLU gate of the Llama MLP over n elements (bf16 or f32, any n, any alignment; 16-byte vectors
+ * when every pointer is 16-byte aligned): out = T(T(silu(gate))*up);
+ * dup = T(dy*T(silu(gate))), dgate = silu_backward(T(dy*up), gate), silu recomputed from gate.
+ * Same fp32 formulas as ATen's CUDA silu / silu_backward (x/(1+exp(-x)), dy*s*(1+x*(1-s))):
+ * bit-identical to the chains silu -> mul and mul, mul, silu_backward. */
+int edb_swiglu_fwd(void* out, const void* gate, const void* up, int64_t n, int dtype, void* stream);
+int edb_swiglu_bwd(void* dgate, void* dup, const void* dy, const void* gate, const void* up,
+                   int64_t n, int dtype, void* stream);
+
 /* Column sums out[c] = sum_r x[r, c] of a [rows, cols] matrix with row stride `ld` (elements):
  * the bias gradients `aten.sum.dim_IntList(dy, [0], True)` of the sharded graph.  bf16 or f32, fp32
  * accumulation in a fixed order (deterministic).  `workspace`: edb_colsum_workspace(cols) bytes. */
