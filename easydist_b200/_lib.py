@@ -111,6 +111,8 @@ SIGNATURES = {
                                  c_void_p, c_int64, c_int64, c_int, c_int, c_void_p]),
     "edb_rms_norm_bwd_workspace": (c_int, [c_int64, POINTER(c_size_t)]),
     "edb_swiglu_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
+    "edb_rope": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64,
+                         _I64P, _I64P, c_int64, c_int, c_int, c_void_p]),
     "edb_swiglu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
                                c_void_p]),
     "edb_colsum": (c_int,[c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int, c_void_p]),

@@ -1307,6 +1307,278 @@ def fuse_swiglu(gm):
     return n, n
 
 
+def _rope_val(nd):
+    v = nd.meta.get("val") if isinstance(nd, Node) else None
+    return v if isinstance(v, torch.Tensor) else None
+
+
+def _bin(nd, target):
+    """The two operands of a binary `target` node without kwargs (no alpha), else None."""
+    return tuple(nd.args) if _call(nd, target) and len(nd.args) == 2 and not nd.kwargs else None
+
+
+def _rope_halves(lo, hi, hd):
+    """Which half of a last dimension of even size hd the slice range [lo, hi) is: 0, 1 or None."""
+    if hd % 2 or not isinstance(hi, int):
+        return None
+    if lo == 0 and hi == hd // 2:
+        return 0
+    return 1 if lo == hd // 2 and hi >= hd else None
+
+
+def _rope_half(nd):
+    """nd == aten.slice.Tensor(src, last dim, ...) of one half of a 4-d src -> (src, 0 | 1)."""
+    if not _call(nd, aten.slice.Tensor) or nd.kwargs or not 4 <= len(nd.args) <= 5:
+        return None
+    src, dim, lo, hi = nd.args[:4]
+    v = _rope_val(src)
+    if v is None or v.dim() != 4 or dim not in (3, -1) or (len(nd.args) == 5 and nd.args[4] != 1):
+        return None
+    w = _rope_halves(lo, hi, int(v.shape[-1]))
+    return None if w is None else (src, w)
+
+
+def _rope_filled(nd):
+    """nd == aten.slice_backward(g, sizes, last dim, ..., 1) filling one half of a 4-d tensor ->
+    (g, 0 | 1)."""
+    if not _call(nd, aten.slice_backward.default) or nd.kwargs or len(nd.args) != 6:
+        return None
+    g, sizes, dim, lo, hi, step = nd.args
+    if len(sizes) != 4 or dim not in (3, -1) or step != 1:
+        return None
+    w = _rope_halves(lo, hi, int(sizes[-1]))
+    return None if w is None else (g, w)
+
+
+def _rope_table(nd, x):
+    """nd if it is a [T, hd/2] table of x's dtype (x: [B, H, T, hd]), else None."""
+    v, xv = _rope_val(nd), _rope_val(x)
+    if v is None or xv is None or v.dtype != xv.dtype \
+            or tuple(v.shape) != (int(xv.shape[2]), int(xv.shape[3]) // 2):
+        return None
+    return nd
+
+
+def _rope_cat_table(nd, x):
+    """nd == aten.cat([c, c], -1) of a table c of x (the rotate_half form) -> c."""
+    if not (_call(nd, aten.cat.default) and len(nd.args) == 2 and nd.args[1] in (-1, 1)
+            and not nd.kwargs and len(nd.args[0]) == 2 and nd.args[0][0] is nd.args[0][1]):
+        return None
+    return _rope_table(nd.args[0][0], x)
+
+
+def _rope_term(m):
+    """m == mul(half slice of src, t), either order -> (slice, src, half, t)."""
+    a = _bin(m, aten.mul.Tensor)
+    for p, q in ((a, a[::-1]) if a else ()):
+        hs = _rope_half(p)
+        if hs is not None and isinstance(q, Node):
+            return p, hs[0], hs[1], q
+    return None
+
+
+def _rope_rotated(rc):
+    """rc == cat([neg(slice(x, second half)), slice(x, first half)], -1) -> (x, [its nodes])."""
+    if not (_call(rc, aten.cat.default) and len(rc.args) == 2 and rc.args[1] in (-1, 3)
+            and not rc.kwargs and len(rc.args[0]) == 2):
+        return None
+    ng, lo = rc.args[0]
+    if not (_call(ng, aten.neg.default) and len(ng.args) == 1 and not ng.kwargs):
+        return None
+    h2, h1 = _rope_half(ng.args[0]), _rope_half(lo)
+    if h2 is None or h1 is None or h2[1] != 1 or h1[1] != 0 or h2[0] is not h1[0]:
+        return None
+    return h2[0], [ng, ng.args[0], lo]
+
+
+def _other(ops, x):
+    """The operand of a binary node's `ops` that is not x (None if x is not one)."""
+    return ops[1] if ops[0] is x else (ops[0] if ops[1] is x else None)
+
+
+def _match_rope_fwd_split(cat):
+    """cat([x1*c - x2*s, x2*c + x1*s], -1) (workloads._rope), x1 / x2 the halves of x."""
+    if not (_call(cat, aten.cat.default) and len(cat.args) == 2 and cat.args[1] in (-1, 3)
+            and not cat.kwargs and len(cat.args[0]) == 2):
+        return None
+    sub, add = cat.args[0]
+    sa, aa = _bin(sub, aten.sub.Tensor), _bin(add, aten.add.Tensor)
+    if sa is None or aa is None:
+        return None
+    terms = [_rope_term(m) for m in sa + aa]
+    if None in terms:
+        return None
+    t1, t2, t3, t4 = terms
+    if t3[2] == 0:
+        t3, t4 = t4, t3
+    x, c, s = t1[1], t1[3], t2[3]
+    if (t1[2], t2[2], t3[2], t4[2]) != (0, 1, 1, 0) or t3[3] is not c or t4[3] is not s \
+            or any(t[1] is not x for t in terms):
+        return None
+    if _rope_table(c, x) is None or _rope_table(s, x) is None:
+        return None
+    muls = list(sa + aa)
+    slices = {t[0] for t in terms}
+    if any(len(nd.users) != 1 for nd in muls + [sub, add]) \
+            or any(set(sl.users) - set(muls) for sl in slices):
+        return None
+    return dict(out=cat, x=x, c=c, s=s, inverse=False, chain=[cat, sub, add, *muls, *slices])
+
+
+def _match_rope_fwd_half(add):
+    """x*cat(c,c) + cat(-x2, x1)*cat(s,s) (the rotate_half form)."""
+    aa = _bin(add, aten.add.Tensor)
+    for m1, m2 in ((aa, aa[::-1]) if aa else ()):
+        r, m = _bin(m2, aten.mul.Tensor), _bin(m1, aten.mul.Tensor)
+        for rc, S in ((r, r[::-1]) if r and m else ()):
+            rot = _rope_rotated(rc)
+            if rot is None or _other(m, rot[0]) is None:
+                continue
+            x = rot[0]
+            C = _other(m, x)
+            c, s = _rope_cat_table(C, x), _rope_cat_table(S, x)
+            chain = [m1, m2, rc, *rot[1]]
+            if c is None or s is None or any(len(nd.users) != 1 for nd in chain):
+                continue
+            return dict(out=add, x=x, c=c, s=s, inverse=False, chain=[add] + chain, dead=[C, S])
+    return None
+
+
+def _match_rope_bwd_split(out):
+    """The autograd backward of the half-split form: with g1 / g2 the halves of the gradient g,
+    slice_backward(g2*c + neg(g1)*s, second half) + slice_backward(g2*s + g1*c, first half)."""
+    oa = _bin(out, aten.add.Tensor)
+    fills = [_rope_filled(nd) for nd in oa] if oa else [None]
+    if None in fills:
+        return None
+    if fills[0][1] == 0:
+        fills = fills[::-1]
+    (d2, w2), (d1, w1) = fills
+    a1, a2 = _bin(d1, aten.add.Tensor), _bin(d2, aten.add.Tensor)
+    if (w2, w1) != (1, 0) or a1 is None or a2 is None:
+        return None
+    t = [_rope_term(m) for m in a1]
+    if None in t:
+        return None
+    if t[0][2] == 0:
+        t = t[::-1]
+    (_, g, wa, s), (_, g1, wb, c) = t
+    if (wa, wb) != (1, 0) or g1 is not g:
+        return None
+    found = None
+    for mn, mc in (a2, a2[::-1]):
+        b = _bin(mn, aten.mul.Tensor)
+        for ng, q in ((b, b[::-1]) if b else ()):
+            hs = _rope_half(ng.args[0]) if _call(ng, aten.neg.default) and len(ng.args) == 1 else None
+            if hs is not None and hs[0] is g and hs[1] == 0 and q is s:
+                found = (mn, mc, ng)
+    if found is None:
+        return None
+    mn, mc, ng = found
+    tc = _rope_term(mc)
+    if tc is None or tc[1] is not g or tc[2] != 1 or tc[3] is not c:
+        return None
+    if _rope_table(c, g) is None or _rope_table(s, g) is None:
+        return None
+    muls = [*a1, mn, mc]
+    slices = {t[0][0], t[1][0], ng.args[0], tc[0]}
+    if any(len(nd.users) != 1 for nd in [*oa, d1, d2, ng, *muls]) \
+            or any(set(sl.users) - set(muls) - {ng} for sl in slices):
+        return None
+    return dict(out=out, x=g, c=c, s=s, inverse=True, chain=[out, *oa, d1, d2, ng, *muls, *slices])
+
+
+def _match_rope_bwd_half(out):
+    """The autograd backward of the rotate_half form: with m = g*cat(s,s),
+    (slice_backward(m2, first half) + slice_backward(neg(m1), second half)) + g*cat(c,c)."""
+    oa = _bin(out, aten.add.Tensor)
+    for A, mc in ((oa, oa[::-1]) if oa else ()):
+        aa, b = _bin(A, aten.add.Tensor), _bin(mc, aten.mul.Tensor)
+        fills = [_rope_filled(nd) for nd in aa] if aa and b else [None]
+        if None in fills:
+            continue
+        if fills[0][1] == 1:
+            fills = fills[::-1]
+        (p0, w0), (p1, w1) = fills
+        if (w0, w1) != (0, 1) or not (_call(p1, aten.neg.default) and len(p1.args) == 1):
+            continue
+        h0, h1 = _rope_half(p0), _rope_half(p1.args[0])
+        if h0 is None or h1 is None or h0[1] != 1 or h1[1] != 0 or h0[0] is not h1[0]:
+            continue
+        m = h0[0]
+        mb = _bin(m, aten.mul.Tensor)
+        for g, S in ((mb, mb[::-1]) if mb else ()):
+            C = _other(b, g)
+            if C is None:
+                continue
+            c, s = _rope_cat_table(C, g), _rope_cat_table(S, g)
+            chain = [A, mc, *aa, p0, p1, p1.args[0]]
+            if c is None or s is None or any(len(nd.users) != 1 for nd in chain) \
+                    or set(m.users) != {p0, p1.args[0]}:
+                continue
+            return dict(out=out, x=g, c=c, s=s, inverse=True, chain=[out, m] + chain, dead=[C, S])
+    return None
+
+
+def fuse_rope(gm):
+    """Rewrite rotary position embeddings onto edb_rope.cu (rope.rope): the half-split chain
+    `cat(x1*c - x2*s, x2*c + x1*s)` (workloads._rope), the rotate_half chain
+    `x*cat(c,c) + cat(-x2, x1)*cat(s,s)` and the autograd backwards of both, each matched on its own
+    (a backward needs only the tables).  x is [B, H, T, hd] and each table a [T, hd/2] node of x's
+    dtype (rotate_half: `cat([c, c], -1)` of one).  The kernel reads x through its strides (the
+    transposed view of the projection output) and writes the layout of the replaced node; a backward
+    result read only by `transpose(1, 2)` -> `clone(contiguous_format)` is written in the clone's
+    [B, T, H, hd] layout and both nodes go.  Chains with an extra reader of an intermediate, or a
+    table of another dtype (type promotion), are left alone.  Returns (forward, backward) counts."""
+    from . import rope
+    graph = gm.graph
+    n_fwd = n_bwd = 0
+    gone = set()
+    for nd in list(graph.nodes):
+        if nd in gone:
+            continue
+        m = None
+        if _call(nd, aten.cat.default):
+            m = _match_rope_fwd_split(nd)
+        elif _call(nd, aten.add.Tensor):
+            m = _match_rope_fwd_half(nd) or _match_rope_bwd_split(nd) or _match_rope_bwd_half(nd)
+        if m is None:
+            continue
+        out, chain = m["out"], list(dict.fromkeys(m["chain"]))
+        target, kw = out, {}
+        if m["inverse"]:
+            tr = _only_user(out)
+            cl = _only_user(tr) if _call(tr, aten.transpose.int) and len(tr.args) == 3 \
+                and sorted(d % 4 for d in tr.args[1:]) == [1, 2] else None
+            if _call(cl, aten.clone.default) and len(cl.args) == 1 \
+                    and cl.kwargs == {"memory_format": torch.contiguous_format}:
+                target, kw = cl, {"transposed": True}
+                chain += [tr, cl]
+        if not kw and _rope_val(out) is not None:
+            kw = {"stride": list(_rope_val(out).stride())}
+        with graph.inserting_before(out):
+            new = graph.call_function(rope.rope, (m["x"], m["c"], m["s"], m["inverse"]), kw)
+        new.meta = dict(target.meta)
+        target.replace_all_uses_with(new)
+        order = {n: i for i, n in enumerate(graph.nodes)}
+        for d in sorted(chain, key=lambda n: -order[n]):
+            assert not d.users, (d, list(d.users))
+            graph.erase_node(d)
+            gone.add(d)
+        for t in dict.fromkeys(m.get("dead", ())):
+            if not t.users:
+                graph.erase_node(t)
+                gone.add(t)
+        if m["inverse"]:
+            n_bwd += 1
+        else:
+            n_fwd += 1
+    if n_fwd or n_bwd:
+        graph.lint()
+        gm.recompile()
+    return n_fwd, n_bwd
+
+
 def fuse_optimizer_updates(gm):
     """The re-inplaced update of torch.optim.SGD(momentum, foreach=True),
         _foreach_mul_(bufs, mu); _foreach_add_(bufs, grads[, alpha=a]); _foreach_add_(params, bufs, alpha=-lr)
@@ -1546,8 +1818,8 @@ def fuse_gemm_epilogues(gm):
 
 def dispatch_compute(gm, counts=None):
     """Route bf16 `aten.mm` / `aten.addmm` nodes to the wgmma GEMM (sharded-op kernel dispatch).
-    `counts` (a dict), when given, receives the (forward, backward) counts of the RMSNorm and SwiGLU
-    rewrites as "rms_norm" and "swiglu"."""
+    `counts` (a dict), when given, receives the (forward, backward) counts of the RMSNorm, SwiGLU and
+    RoPE rewrites as "rms_norm", "swiglu" and "rope"."""
     import os
     from . import gemm, norm
     native_ln = os.environ.get("EDB_NATIVE_LN", "1") == "1"
@@ -1560,7 +1832,8 @@ def dispatch_compute(gm, counts=None):
     # before the sum.dim_IntList retargeting below, which would otherwise claim the dw sums
     counts["rms_norm"] = fuse_rms_norm(gm) if os.environ.get("EDB_NATIVE_RMS", "1") == "1" else (0, 0)
     counts["swiglu"] = fuse_swiglu(gm) if os.environ.get("EDB_NATIVE_SWIGLU", "1") == "1" else (0, 0)
-    n += sum(counts["rms_norm"]) + sum(counts["swiglu"])
+    counts["rope"] = fuse_rope(gm) if os.environ.get("EDB_NATIVE_ROPE", "1") == "1" else (0, 0)
+    n += sum(counts["rms_norm"]) + sum(counts["swiglu"]) + sum(counts["rope"])
     for node in gm.graph.nodes:
         if node.op != "call_function":
             continue

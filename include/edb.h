@@ -359,6 +359,19 @@ int edb_swiglu_fwd(void* out, const void* gate, const void* up, int64_t n, int d
 int edb_swiglu_bwd(void* dgate, void* dup, const void* dy, const void* gate, const void* up,
                    int64_t n, int dtype, void* stream);
 
+/* Rotary position embedding of a [B, H, T, 2*half] tensor x with [T, half] tables cos / sin (rows
+ * `table_stride_t` elements apart, broadcast over b and h); x, y addressed through their (b, h, t)
+ * element strides x_strides[3], y_strides[3], last dimension contiguous; bf16 or f32 (`dtype`); y
+ * must not overlap x.  With x1, x2 the halves of the last dimension and T() the rounding to dtype:
+ *   y1 = T(T(x1*c) - T(x2*s')),  y2 = T(T(x2*c) + T(x1*s')),  s' = inverse ? -s : s
+ * (inverse: -0 results become +0).  Bit-identical to the half-split chain cat(x1*c - x2*s,
+ * x2*c + x1*s), the rotate_half chain x*cat(c,c) + cat(-x2,x1)*cat(s,s), and their autograd
+ * backwards (inverse = 1).  16-byte vectors when `half`, the strides and every pointer allow it.
+ * half in 1..256 (head dim <= 512) and T*half <= 2^30, else EDB_E_UNSUPPORTED. */
+int edb_rope(void* y, const void* x, const void* cos, const void* sin, int64_t B, int64_t H,
+             int64_t T, int64_t half, const int64_t* x_strides, const int64_t* y_strides,
+             int64_t table_stride_t, int inverse, int dtype, void* stream);
+
 /* Column sums out[c] = sum_r x[r, c] of a [rows, cols] matrix with row stride `ld` (elements):
  * the bias gradients `aten.sum.dim_IntList(dy, [0], True)` of the sharded graph.  bf16 or f32, fp32
  * accumulation in a fixed order (deterministic).  `workspace`: edb_colsum_workspace(cols) bytes. */
