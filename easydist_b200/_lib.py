@@ -124,6 +124,11 @@ SIGNATURES = {
                                       c_void_p]),
     "edb_sgd_momentum": (c_int, [c_int, c_void_p, c_void_p, c_void_p, _I64P, c_float, c_float, c_float,
                                  c_int, c_void_p]),
+    "edb_sgd_momentum_scaled": (c_int, [c_int, c_void_p, c_void_p, c_void_p, _I64P, c_float, c_float,
+                                        c_float, c_void_p, c_int, c_void_p]),
+    "edb_grad_sumsq": (c_int, [c_int, c_void_p, _I64P, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "edb_grad_sumsq_workspace": (c_int, [c_int, _I64P, c_int, POINTER(c_size_t)]),
+    "edb_multi_scale_": (c_int, [c_int, c_void_p, _I64P, c_void_p, c_int, c_void_p]),
     "edb_set_option": (c_int, [c_char_p, c_int64]),
     "edb_get_option": (c_int, [c_char_p, POINTER(c_int64)]),
     "edb_launch_count": (c_uint64, []),

@@ -34,6 +34,7 @@ struct OptDesc {
   int first_chunk[kOptMaxTensors + 1];  // prefix sum of chunks per tensor
   int n;
   float mu, grad_alpha, neg_lr;
+  const void* grad_scale;  // kScaled: device scalar c of the storage dtype
 };
 static_assert(sizeof(OptDesc) <= 16 * 1024, "descriptor must fit the kernel parameter space");
 
@@ -47,7 +48,8 @@ __device__ __forceinline__ void sgd_elem(float& p, float g, float& m, float mu, 
   p = OptT<T>::rnd(fmaf(nlr, m, p));               // _foreach_add_(params, bufs, alpha=-lr)
 }
 
-template <typename T>
+// kScaled: g' = T(g*c) first, the rounding of the in-place `mul_(g, c)` of gradient clipping
+template <typename T, bool kScaled>
 __global__ void __launch_bounds__(kOptThreads)
     k_sgd_momentum(const __grid_constant__ OptDesc d) {
   constexpr int EPV = OptT<T>::EPV;
@@ -66,6 +68,7 @@ __global__ void __launch_bounds__(kOptThreads)
   const uint4* gv = reinterpret_cast<const uint4*>(t.g);
   uint4* mv = reinterpret_cast<uint4*>(t.m);
   const float mu = d.mu, ga = d.grad_alpha, nlr = d.neg_lr;
+  const float gc = kScaled ? OptT<T>::ld(reinterpret_cast<const T*>(d.grad_scale)) : 1.f;
   uint4 rp[4], rg[4], rm[4];
 #pragma unroll
   for (int u = 0; u < 4; ++u) {
@@ -84,6 +87,10 @@ __global__ void __launch_bounds__(kOptThreads)
       OptT<T>::unpack(rp[u], fp);
       OptT<T>::unpack(rg[u], fg);
       OptT<T>::unpack(rm[u], fm);
+      if (kScaled) {
+#pragma unroll
+        for (int e = 0; e < EPV; ++e) fg[e] = OptT<T>::rnd(__fmul_rn(fg[e], gc));
+      }
 #pragma unroll
       for (int e = 0; e < EPV; ++e) sgd_elem<T>(fp[e], fg[e], fm[e], mu, ga, nlr);
       mv[i] = OptT<T>::pack(fm);
@@ -97,7 +104,9 @@ __global__ void __launch_bounds__(kOptThreads)
     T* p = reinterpret_cast<T*>(t.p) + i;
     T* m = reinterpret_cast<T*>(t.m) + i;
     float fp = OptT<T>::ld(p), fm = OptT<T>::ld(m);
-    sgd_elem<T>(fp, OptT<T>::ld(reinterpret_cast<const T*>(t.g) + i), fm, mu, ga, nlr);
+    float fg = OptT<T>::ld(reinterpret_cast<const T*>(t.g) + i);
+    if (kScaled) fg = OptT<T>::rnd(__fmul_rn(fg, gc));
+    sgd_elem<T>(fp, fg, fm, mu, ga, nlr);
     OptT<T>::st(m, fm);
     OptT<T>::st(p, fp);
   }
@@ -109,9 +118,9 @@ using namespace edb;
 
 extern "C" {
 
-int edb_sgd_momentum(int n, void* const* params, const void* const* grads, void* const* bufs,
-                     const int64_t* numels, float mu, float grad_alpha, float neg_lr, int dtype,
-                     void* stream) {
+static int sgd_momentum(int n, void* const* params, const void* const* grads, void* const* bufs,
+                        const int64_t* numels, float mu, float grad_alpha, float neg_lr,
+                        const void* grad_scale, int dtype, void* stream) {
   if (n <= 0) return EDB_OK;
   if (dtype != EDB_BF16 && dtype != EDB_F32)
     return set_error(EDB_E_UNSUPPORTED, "edb_sgd_momentum: dtype %d", dtype);
@@ -128,6 +137,7 @@ int edb_sgd_momentum(int n, void* const* params, const void* const* grads, void*
     d.mu = mu;
     d.grad_alpha = grad_alpha;
     d.neg_lr = neg_lr;
+    d.grad_scale = grad_scale;
     int k = 0;
     int64_t chunks = 0;
     d.first_chunk[0] = 0;
@@ -152,11 +162,32 @@ int edb_sgd_momentum(int n, void* const* params, const void* const* grads, void*
       if (done < n) return set_error(EDB_E_UNSUPPORTED, "edb_sgd_momentum: tensor %d too large", done);
       continue;
     }
-    if (dtype == EDB_BF16) k_sgd_momentum<__nv_bfloat16><<<(unsigned)chunks, kOptThreads, 0, st>>>(d);
-    else k_sgd_momentum<float><<<(unsigned)chunks, kOptThreads, 0, st>>>(d);
+    const unsigned grid = (unsigned)chunks;
+    if (dtype == EDB_BF16) {
+      if (grad_scale) k_sgd_momentum<__nv_bfloat16, true><<<grid, kOptThreads, 0, st>>>(d);
+      else k_sgd_momentum<__nv_bfloat16, false><<<grid, kOptThreads, 0, st>>>(d);
+    } else {
+      if (grad_scale) k_sgd_momentum<float, true><<<grid, kOptThreads, 0, st>>>(d);
+      else k_sgd_momentum<float, false><<<grid, kOptThreads, 0, st>>>(d);
+    }
     count_launch();
   }
   return cuda_check(cudaGetLastError(), "k_sgd_momentum launch");
+}
+
+int edb_sgd_momentum(int n, void* const* params, const void* const* grads, void* const* bufs,
+                     const int64_t* numels, float mu, float grad_alpha, float neg_lr, int dtype,
+                     void* stream) {
+  return sgd_momentum(n, params, grads, bufs, numels, mu, grad_alpha, neg_lr, nullptr, dtype, stream);
+}
+
+int edb_sgd_momentum_scaled(int n, void* const* params, const void* const* grads, void* const* bufs,
+                            const int64_t* numels, float mu, float grad_alpha, float neg_lr,
+                            const void* grad_scale, int dtype, void* stream) {
+  if (n > 0 && grad_scale == nullptr)
+    return set_error(EDB_E_INVALID, "edb_sgd_momentum_scaled: grad_scale is NULL");
+  return sgd_momentum(n, params, grads, bufs, numels, mu, grad_alpha, neg_lr, grad_scale, dtype,
+                      stream);
 }
 
 }  // extern "C"

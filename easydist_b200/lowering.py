@@ -398,6 +398,89 @@ def _bucket_small_grads(gm, io, ranks, small, region, ops):
         g.replace_all_uses_with(piece, delete_user_cb=lambda u: u not in own)
 
 
+def _is_norm2(nd):
+    return _call(nd, aten.linalg_vector_norm.default) and len(nd.args) == 2 and not nd.kwargs \
+        and nd.args[1] == 2
+
+
+def _clip_coef(total):
+    """The coefficient tail of clip_grad_norm_ behind the total norm `total`:
+    clamp(mul(reciprocal(add(total, eps)), max_norm), None, 1.0) -> (clamp node, tail nodes) or None."""
+    add = _only_user(total)
+    if not (_call(add, aten.add.Tensor) and add.args[0] is total and not add.kwargs
+            and isinstance(add.args[1], (int, float))):
+        return None
+    rec = _only_user(add)
+    if not (_call(rec, aten.reciprocal.default) and not rec.kwargs):
+        return None
+    mul = _only_user(rec)
+    if not (_call(mul, aten.mul.Tensor) and mul.args[0] is rec and not mul.kwargs
+            and isinstance(mul.args[1], (int, float))):
+        return None
+    clamp = _only_user(mul)
+    if not (_call(clamp, aten.clamp.default) and clamp.args[0] is mul and not clamp.kwargs
+            and tuple(clamp.args[1:]) == (None, 1.0)):
+        return None
+    return clamp, (add, rec, mul)
+
+
+def _match_clip(gm):
+    """The chains `torch.nn.utils.clip_grad_norm_(params, max_norm)` traces to (norm_type 2,
+    error_if_nonfinite=False, foreach=None):
+        n_i = linalg_vector_norm(g_i, 2.0)  (each read only by the stack)
+        total = linalg_vector_norm(stack([n_1 .. n_T]), 2.0)
+        coef = clamp(max_norm * reciprocal(total + 1e-6), max=1.0)
+        mul_(g_i, coef) ...
+    -> list of dicts: norms, stack, total, clamp, tail (the ops between total and clamp)."""
+    out = []
+    for total in gm.graph.nodes:
+        if not _is_norm2(total) or not _call(total.args[0], aten.stack.default):
+            continue
+        stack = total.args[0]
+        norms = stack.args[0]
+        if len(stack.users) != 1 or (stack.args[1:] or [0])[0] != 0 or stack.kwargs or not norms \
+                or len(set(norms)) != len(norms) \
+                or not all(_is_norm2(nd) and len(nd.users) == 1 for nd in norms):
+            continue
+        coef = _clip_coef(total)
+        if coef is None:
+            continue
+        out.append(dict(norms=list(norms), stack=stack, total=total, clamp=coef[0], tail=coef[1]))
+    return out
+
+
+def _clip_sharded_norms(gm, chain, replicated, ranks, ops):
+    """zero2/zero3: the per-gradient norms of one clip chain from the local gradients (flat 1/n shards
+    or, for `replicated` entries, the full bucketed gradient).  Sharded entries: Σx² of the shard per
+    tensor (clip.grad_sumsq), all-reduce(sum) of that [S] fp32 vector, sqrt, cast to the gradient dtype
+    -- the same bits on every rank.  Replicated entries are complete on every rank: their norms are
+    taken locally (counting them in the all-reduce would add them n times)."""
+    from . import clip
+    graph = gm.graph
+    norms, stack = chain["norms"], chain["stack"]
+    groups = ([i for i, nd in enumerate(norms) if nd not in replicated],
+              [i for i, nd in enumerate(norms) if nd in replicated])
+    with graph.inserting_before(stack):
+        for k, idx in enumerate(groups):
+            if not idx:
+                continue
+            xs = [norms[i].args[0] for i in idx]
+            if k == 0:
+                ss = graph.call_function(clip.grad_sumsq, (xs,))
+                s = graph.call_function(ops.all_reduce_start, args=(ss, "sum", list(ranks)))
+                e = graph.call_function(ops.all_reduce_end, args=(s, "sum", list(ranks)))
+                r = graph.call_function(aten.sqrt.default, (e,))
+                vec = graph.call_function(aten._to_copy.default, (r,),
+                                          {"dtype": norms[idx[0]].meta["val"].dtype})
+            else:
+                vec = graph.call_function(clip.grad_norms, (xs,))
+            for j, i in enumerate(idx):
+                sel = graph.call_function(aten.select.int, (vec, 0, j))
+                norms[i].replace_all_uses_with(sel)
+    for nd in norms:
+        graph.erase_node(nd)
+
+
 def transform_fsdp(gm, io, ranks, my_index, shard_param, ops=_default_ops, bucket_numel=0):
     """zero2 (shard_param=False) / zero3 (True), compile_dp.py:82-198: gradients are flattened and
     reduce-scattered(avg), optimizer states (and, for zero3, parameters) live as flat 1/n shards;
@@ -411,9 +494,20 @@ def transform_fsdp(gm, io, ranks, my_index, shard_param, ops=_default_ops, bucke
     region = optimizer_region(gm, io)
     region_set = set(region)
     allowed = _optimizer_elementwise_ops()
+    # gradient-norm clipping: the per-gradient norms are recomputed from the shards below; the tail
+    # (stack, total norm, clamp) runs on replicated [T] values and each mul_ on one gradient shard
+    grad_of = {g: ph for ph, g in zip(io.param_ph, io.final_grads) if isinstance(g, Node)}
+    clips, clip_nodes = [], set()
+    for ch in _match_clip(gm):
+        if all(nd.args[0] in grad_of for nd in ch["norms"]):
+            ch["params"] = [grad_of[nd.args[0]] for nd in ch["norms"]]
+            clips.append(ch)
+            clip_nodes.update(ch["norms"], (ch["stack"], ch["total"], ch["clamp"]))
+            clip_nodes.update(u for u in ch["clamp"].users if _call(u, aten.mul_.Tensor)
+                              and len(u.args) == 2 and u.args[1] is ch["clamp"] and not u.kwargs)
     for node in region:
         if node.op == "call_function" and node.target not in allowed and \
-                node.target not in ops.CUSTOM_FUNCS:
+                node.target not in ops.CUSTOM_FUNCS and node not in clip_nodes:
             raise NotImplementedError(
                 f"zero2/zero3: optimizer op {node.target} is not elementwise over (param, grad, "
                 f"state); cannot run it on flat shards")
@@ -442,6 +536,9 @@ def transform_fsdp(gm, io, ranks, my_index, shard_param, ops=_default_ops, bucke
         with graph.inserting_after(s):
             e = graph.call_function(ops.reduce_scatter_end, args=(s, "avg", 0, ranks))
         g.replace_all_uses_with(e, delete_user_cb=lambda u: u is not f)
+    for ch in clips:
+        _clip_sharded_norms(gm, ch, {nd for nd, ph in zip(ch["norms"], ch["params"]) if ph in small},
+                            ranks, ops)
 
     # (2) parameters
     for ph in io.param_ph:
@@ -1635,6 +1732,114 @@ def fuse_optimizer_updates(gm):
     return n
 
 
+# ops whose result shares memory with their first argument (an in-place write through one is seen
+# through all of them)
+_ALIAS_OPS = (aten.t.default, aten.view.default, aten._unsafe_view.default, aten.transpose.int,
+              aten.permute.default, aten.alias.default, aten.detach.default, aten.slice.Tensor,
+              aten.select.int, aten.flatten.using_ints, aten.reshape.default, aten.expand.default,
+              aten.unsqueeze.default, aten.squeeze.dim, aten.as_strided.default)
+
+
+def _memory_readers(x):
+    """Every non-view node that reads memory of `x`: through x, the views x was taken from, and any
+    view of those."""
+    root = x
+    while _call(root, *_ALIAS_OPS):
+        root = root.args[0]
+    readers, frontier, seen = [], [root], {root}
+    while frontier:
+        nd = frontier.pop()
+        for u in nd.users:
+            if u in seen:
+                continue
+            seen.add(u)
+            if _call(u, *_ALIAS_OPS) and u.args[0] is nd:
+                frontier.append(u)
+            else:
+                readers.append(u)
+    return readers
+
+
+def _fold_clip_scale(gm, clamp):
+    """The in-place `mul_(g_i, clamp)` nodes of one clip coefficient.  When one fused SGD node reads
+    exactly their results and nothing after a mul_ reads g_i's memory other than through it, the
+    scale moves into that node (`grad_scale=`, g_i is no longer written); otherwise they become one
+    `clip.scale_` node.  A mul_ on a tensor of another dtype than the coefficient (type promotion) is
+    left alone.  -> number of mul_ nodes replaced."""
+    from . import clip, optim
+    graph = gm.graph
+    dt = clamp.meta["val"].dtype if isinstance(clamp.meta.get("val"), torch.Tensor) else None
+    muls = [u for u in clamp.users if _call(u, aten.mul_.Tensor) and len(u.args) == 2
+            and u.args[1] is clamp and u.args[0] is not clamp and not u.kwargs
+            and isinstance(u.args[0].meta.get("val"), torch.Tensor)
+            and u.args[0].meta["val"].dtype == dt]
+    if not muls or len({m.args[0] for m in muls}) != len(muls):
+        return 0
+    pos = {nd: i for i, nd in enumerate(graph.nodes)}
+    muls.sort(key=lambda m: pos[m])
+    group = set(muls)
+    users = {u for m in muls for u in m.users}
+    sgd = next(iter(users)) if len(users) == 1 else None
+    if _call(sgd, optim.sgd_momentum_) and "grad_scale" not in sgd.kwargs \
+            and all(len(m.users) == 1 for m in muls) and set(sgd.args[1]) == group \
+            and len(sgd.args[1]) == len(muls) \
+            and not any(pos[r] > pos[m] and r not in group
+                        for m in muls for r in _memory_readers(m.args[0])):
+        args = list(sgd.args)
+        args[1] = [m.args[0] for m in args[1]]
+        sgd.args = tuple(args)
+        sgd.kwargs = dict(sgd.kwargs, grad_scale=clamp)
+        for m in muls:
+            graph.erase_node(m)
+        return len(muls)
+    # one scale_ in front of the first mul_: nothing between the first and the last may read the
+    # memory of a gradient whose mul_ comes later
+    first = pos[muls[0]]
+    for m in muls:
+        if any(first < pos[r] < pos[m] and r not in group for r in _memory_readers(m.args[0])):
+            return 0
+    with graph.inserting_before(muls[0]):
+        graph.call_function(clip.scale_, ([m.args[0] for m in muls], clamp))
+    for m in muls:
+        m.replace_all_uses_with(m.args[0])
+        graph.erase_node(m)
+    return len(muls)
+
+
+def fuse_grad_clip(gm):
+    """clip_grad_norm_(params, max_norm) (norm_type 2) on native multi-tensor kernels: the T norm
+    nodes and their stack become one `clip.grad_norms` node (one read of every gradient), and the T
+    in-place `mul_(g_i, coef)` nodes fold into the fused SGD (`sgd_momentum_(..., grad_scale=coef)`)
+    or become one `clip.scale_` node (see _fold_clip_scale).  In zero2/zero3 graphs the norms were
+    already recomputed from the shards (transform_fsdp); only the scale is folded there.
+    -> (norm nodes replaced, scale nodes replaced)."""
+    from . import clip
+    graph = gm.graph
+    n_norm = n_scale = 0
+    for ch in _match_clip(gm):
+        norms, stack = ch["norms"], ch["stack"]
+        dts = {nd.meta["val"].dtype for nd in norms if isinstance(nd.meta.get("val"), torch.Tensor)}
+        if len(dts) != 1 or any(not isinstance(nd.args[0].meta.get("val"), torch.Tensor)
+                                or nd.args[0].meta["val"].dtype not in dts for nd in norms):
+            continue
+        with graph.inserting_before(stack):
+            gn = graph.call_function(clip.grad_norms, ([nd.args[0] for nd in norms],))
+        gn.meta = dict(stack.meta)
+        stack.replace_all_uses_with(gn)
+        graph.erase_node(stack)
+        for nd in norms:
+            graph.erase_node(nd)
+        n_norm += len(norms)
+    for total in [nd for nd in graph.nodes if _is_norm2(nd)]:
+        coef = _clip_coef(total)
+        if coef is not None:
+            n_scale += _fold_clip_scale(gm, coef[0])
+    if n_norm or n_scale:
+        graph.lint()
+        gm.recompile()
+    return n_norm, n_scale
+
+
 _VIEW_ONLY = None
 
 
@@ -1819,7 +2024,8 @@ def fuse_gemm_epilogues(gm):
 def dispatch_compute(gm, counts=None):
     """Route bf16 `aten.mm` / `aten.addmm` nodes to the wgmma GEMM (sharded-op kernel dispatch).
     `counts` (a dict), when given, receives the (forward, backward) counts of the RMSNorm, SwiGLU and
-    RoPE rewrites as "rms_norm", "swiglu" and "rope"."""
+    RoPE rewrites as "rms_norm", "swiglu" and "rope", and the (norm, scale) counts of the gradient
+    clipping rewrite as "clip"."""
     import os
     from . import gemm, norm
     native_ln = os.environ.get("EDB_NATIVE_LN", "1") == "1"
@@ -1833,7 +2039,9 @@ def dispatch_compute(gm, counts=None):
     counts["rms_norm"] = fuse_rms_norm(gm) if os.environ.get("EDB_NATIVE_RMS", "1") == "1" else (0, 0)
     counts["swiglu"] = fuse_swiglu(gm) if os.environ.get("EDB_NATIVE_SWIGLU", "1") == "1" else (0, 0)
     counts["rope"] = fuse_rope(gm) if os.environ.get("EDB_NATIVE_ROPE", "1") == "1" else (0, 0)
-    n += sum(counts["rms_norm"]) + sum(counts["swiglu"]) + sum(counts["rope"])
+    # behind fuse_optimizer_updates: the clip scale folds into the fused SGD node
+    counts["clip"] = fuse_grad_clip(gm) if os.environ.get("EDB_NATIVE_CLIP", "1") == "1" else (0, 0)
+    n += sum(counts["rms_norm"]) + sum(counts["swiglu"]) + sum(counts["rope"]) + sum(counts["clip"])
     for node in gm.graph.nodes:
         if node.op != "call_function":
             continue

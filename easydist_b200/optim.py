@@ -42,38 +42,54 @@ def _tensor_ok(p, g, m, dt):
     return not ((p.data_ptr() | g.data_ptr() | m.data_ptr()) & 15)
 
 
-def _aten(params, grads, bufs, mu, grad_alpha, neg_lr):
+def _scale_ok(c, p):
+    return c.dtype == p.dtype and c.device == p.device and c.numel() == 1
+
+
+def _aten(params, grads, bufs, mu, grad_alpha, neg_lr, grad_scale=None):
+    if grad_scale is not None:  # clip_grad_norm_'s mul_(g, coef), without writing g
+        grads = [aten.mul.Tensor(g, grad_scale) for g in grads]
     aten._foreach_mul_.Scalar(bufs, mu)
     aten._foreach_add_.List(bufs, grads, alpha=grad_alpha)
     aten._foreach_add_.List(params, bufs, alpha=neg_lr)
 
 
 @has_side_effect
-def sgd_momentum_(params, grads, bufs, mu, grad_alpha, neg_lr):
+def sgd_momentum_(params, grads, bufs, mu, grad_alpha, neg_lr, grad_scale=None):
     """In place: bufs = mu*bufs + grad_alpha*grads; params += neg_lr*bufs (per tensor).  Tensors the
     kernel's contract does not cover (other dtypes, views that are not 16-byte aligned, e.g. slices
-    of a gradient bucket) take the three ATen ops; both groups are counted."""
+    of a gradient bucket) take the three ATen ops; both groups are counted.
+
+    grad_scale (a one-element tensor of the parameters' dtype): the update uses T(g*grad_scale), the
+    rounding of gradient clipping's `mul_(g, grad_scale)`; the gradients themselves are not written."""
     if not params or len(params) != len(grads) or len(params) != len(bufs):
         raise ValueError("sgd_momentum_: params, grads and bufs must be lists of equal length")
     if isinstance(params[0], FakeTensor):
-        return _aten(params, grads, bufs, mu, grad_alpha, neg_lr)
+        return _aten(params, grads, bufs, mu, grad_alpha, neg_lr, grad_scale)
     native = {}
     rest = []
     for i, (p, g, m) in enumerate(zip(params, grads, bufs)):
-        if p.dtype in _DT and _tensor_ok(p, g, m, p.dtype):
+        if p.dtype in _DT and _tensor_ok(p, g, m, p.dtype) and \
+                (grad_scale is None or _scale_ok(grad_scale, p)):
             native.setdefault(p.dtype, []).append(i)
         else:
             rest.append(i)
     if rest:
         _stats["aten_sgd"] += 1
         _aten([params[i] for i in rest], [grads[i] for i in rest], [bufs[i] for i in rest], mu,
-              grad_alpha, neg_lr)
+              grad_alpha, neg_lr, grad_scale)
     for dt, idx in native.items():
         lib = _lib.load()
         ps, gs, ms = [params[i] for i in idx], [grads[i] for i in idx], [bufs[i] for i in idx]
         stream = torch.cuda.current_stream(ps[0].device).cuda_stream
-        check(lib.edb_sgd_momentum(len(ps), _ptr_array(ps), _ptr_array(gs), _ptr_array(ms),
-                                   i64_array([p.numel() for p in ps]), float(mu), float(grad_alpha),
-                                   float(neg_lr), _DT[dt], stream))
+        if grad_scale is None:
+            check(lib.edb_sgd_momentum(len(ps), _ptr_array(ps), _ptr_array(gs), _ptr_array(ms),
+                                       i64_array([p.numel() for p in ps]), float(mu),
+                                       float(grad_alpha), float(neg_lr), _DT[dt], stream))
+        else:
+            check(lib.edb_sgd_momentum_scaled(len(ps), _ptr_array(ps), _ptr_array(gs), _ptr_array(ms),
+                                              i64_array([p.numel() for p in ps]), float(mu),
+                                              float(grad_alpha), float(neg_lr), grad_scale.data_ptr(),
+                                              _DT[dt], stream))
         _stats["edb_sgd"] += 1
     return None

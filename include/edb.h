@@ -406,6 +406,31 @@ int edb_cross_entropy_bwd(void* dlogits, int64_t ld_out, const void* logits, int
 int edb_sgd_momentum(int n, void* const* params, const void* const* grads, void* const* bufs,
                      const int64_t* numels, float mu, float grad_alpha, float neg_lr, int dtype,
                      void* stream);
+/* The same step on the clipped gradient: g' = T(g*c) with c = *grad_scale (a device scalar of
+ * `dtype`), the rounding of clip_grad_norm_'s in-place `mul_(g, c)`, then the three ops above; g
+ * itself is not written.  Bit-identical to mul_ followed by the unfused SGD. */
+int edb_sgd_momentum_scaled(int n, void* const* params, const void* const* grads, void* const* bufs,
+                            const int64_t* numels, float mu, float grad_alpha, float neg_lr,
+                            const void* grad_scale, int dtype, void* stream);
+
+/* Gradient-norm clipping (torch.nn.utils.clip_grad_norm_, norm_type 2) over n tensors given as host
+ * arrays of device pointers and element counts, all of `dtype` bf16 or f32, each a dense span of
+ * numel elements (any order: a permuted dense view is read as its storage); any alignment (16-byte
+ * vectors where the address allows).
+ * edb_grad_sumsq: out[i] = sum of g_i^2 in fp32 (EDB_SUMSQ_RAW, out: n floats) or T(sqrtf(that sum))
+ * (EDB_SUMSQ_NORM, out: n values of `dtype`, what linalg_vector_norm(g_i, 2) returns).  One fp32
+ * partial per chunk of 8192 (bf16) / 4096 (f32) elements of one tensor, then each tensor's partials
+ * added in index order: deterministic, no atomics, no host synchronisation.  `workspace`:
+ * edb_grad_sumsq_workspace(n, numels, dtype) bytes.
+ * edb_multi_scale_: g_i = T(g_i*c) in place, c = *coef (device scalar of `dtype`): bit-identical to
+ * the per-tensor `mul_(g_i, c)`.  Malformed arguments return an error without a launch. */
+#define EDB_SUMSQ_RAW 0
+#define EDB_SUMSQ_NORM 1
+int edb_grad_sumsq(int n, const void* const* grads, const int64_t* numels, void* out,
+                   void* workspace, int mode, int dtype, void* stream);
+int edb_grad_sumsq_workspace(int n, const int64_t* numels, int dtype, size_t* bytes_out);
+int edb_multi_scale_(int n, void* const* grads, const int64_t* numels, const void* coef, int dtype,
+                     void* stream);
 
 /* ---- options / introspection --------------------------------------------------------------- */
 
