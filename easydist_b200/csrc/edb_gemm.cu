@@ -1030,6 +1030,228 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
   }
 }
 
+// ---- k_gemm2_bf16: the plain single-GPU GEMM ---------------------------------------------------------
+//
+// C = A.B (+ bias, + fused epilogue) for launches that carry nothing else: no split-K, no prefetch
+// CTAs, no push, 128 x 256 tiles.  Same tile, same smem ring, same MMA order per output element and
+// the same epilogue arithmetic as k_gemm_bf16<256, .., MODE_PLAIN>, so the bits are the same; what
+// differs is how the CTA is organised:
+//   * 384 threads: warpgroup 0 produces (one lane issues TMA) and shrinks to 40 registers per
+//     thread, warpgroups 1 and 2 consume and grow to 232: the 128 accumulator registers plus the
+//     epilogue's temporaries fit, where the 168 of a 288-thread CTA spill;
+//   * each consumer warpgroup stores its own 64 rows: 64 x 64 staging buffers, a 128-thread named
+//     barrier and an elected thread of its own.  The warpgroups never wait for each other after the
+//     main loop, so one may be storing while the other still multiplies.
+// (CTA pairs that multicast their shared B tile were measured on top of this and were slower on
+// most shapes of the GPT-2 step: DESIGN.md §6.  L2 operand traffic is not what limits this kernel.)
+constexpr int kGemm2Threads = 384;
+constexpr int kGemm2EpiBufBytes = 64 * 64 * 2;  // one 64 x 64 bf16 store box (128B swizzle)
+
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+// the two consumer warpgroups' named barriers (ids 1 and 2)
+__device__ __forceinline__ void wg_bar_sync(int wg) {
+  if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
+  else asm volatile("bar.sync 2, 128;" ::: "memory");
+}
+// mbar_wait for a kernel whose roles change their register budget: with a trap inside a role ptxas
+// allocates the whole kernel at the launch-time budget (the 232-register consumers then spill like
+// 168-register ones).  So the watchdog only reports here, the role winds down, and the kernel traps
+// in the code all roles share.
+__device__ __forceinline__ bool mbar_wait_ok(uint64_t* bar, uint32_t parity) {
+  const uint32_t addr = smem_u32(bar);
+  if (mbar_try_wait(addr, parity)) return true;
+  const uint64_t t0 = globaltimer_ns();
+  uint32_t spins = 0;
+  while (!mbar_try_wait(addr, parity)) {
+    if ((++spins & 0xfff) == 0 && globaltimer_ns() - t0 > 4000000000ull) return false;
+  }
+  return true;
+}
+
+template <bool A_KMAJOR, bool B_KMAJOR>
+__global__ void __launch_bounds__(kGemm2Threads, 1)
+    k_gemm2_bf16(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const __grid_constant__ CUtensorMap tmap_c, const GemmParams p) {
+  constexpr int BN = 256;
+  using Cfg = TileCfg<BN>;
+  constexpr int kStages = Cfg::kStages;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* smem_a = smem;
+  uint8_t* smem_b = smem + kStages * kSmemABytes;
+  uint8_t* smem_epi = smem + kStages * Cfg::kStageBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_epi + Cfg::kEpiBufs * Cfg::kEpiBufBytes);
+  uint64_t* empty_bar = full_bar + kStages;
+
+  const int wgi = threadIdx.x >> 7;
+  const int k_blocks = (p.K + BK - 1) / BK;
+  // tile t = (t % m_tiles, t / m_tiles); CTA c takes tiles c, c + grid, ... as k_gemm_bf16 does
+  const int mt = p.m_tiles;
+  const int num_units = mt * p.n_tiles;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  bool ok = true;  // false: a barrier wait ran into the watchdog
+  if (wgi == 0) {
+    // ===== TMA producer =====
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      prefetch_tmap(&tmap_a);
+      prefetch_tmap(&tmap_b);
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int u = blockIdx.x; ok && u < num_units; u += gridDim.x) {
+        const int m_blk = u % mt, n_blk = u / mt;
+        for (int kb = 0; kb < k_blocks; ++kb) {
+          if (!(ok = mbar_wait_ok(&empty_bar[stage], phase ^ 1))) break;
+          uint8_t* sa = smem_a + stage * kSmemABytes;
+          uint8_t* sb = smem_b + stage * Cfg::kSmemBBytes;
+          mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+          if (A_KMAJOR) {
+            tma_load_2d(&tmap_a, &full_bar[stage], sa, kb * BK, m_blk * BM);
+          } else {
+#pragma unroll
+            for (int h = 0; h < BM / 64; ++h)
+              tma_load_2d(&tmap_a, &full_bar[stage], sa + h * (64 * BK * 2), m_blk * BM + h * 64,
+                          kb * BK);
+          }
+          if (B_KMAJOR) {
+            tma_load_2d(&tmap_b, &full_bar[stage], sb, kb * BK, n_blk * BN);
+          } else {
+#pragma unroll
+            for (int h = 0; h < BN / 64; ++h)
+              tma_load_2d(&tmap_b, &full_bar[stage], sb + h * (64 * BK * 2), n_blk * BN + h * 64,
+                          kb * BK);
+          }
+          if (++stage == kStages) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+  } else {
+    // ===== consumer warpgroups =====
+    setmaxnreg_inc<232>();
+    const int wg = wgi - 1;
+    const int tid = threadIdx.x & 127;
+    const int frag_row = 16 * (tid >> 5) + ((tid & 31) >> 2);  // + 8 for the odd register pairs
+    const int frag_col = 2 * (tid & 3);
+    const int row0 = wg * 64 + frag_row;  // tile row of h = 0
+    const bool issuer = (tid == 0);       // owns this warpgroup's TMA-store bulk groups
+    uint8_t* epi = smem_epi + wg * (2 * kGemm2EpiBufBytes);
+    if (issuer) prefetch_tmap(&tmap_c);
+    const int epi_op = p.epi_op;
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    int ebuf = 0;
+    for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
+      const int m_blk = u % mt, n_blk = u / mt;
+      int prev = -1;
+      for (int kb = 0; kb < k_blocks; ++kb) {
+        if (!(ok = mbar_wait_ok(&full_bar[stage], phase))) break;
+        wgmma_fence();
+        mma_k_block<BN, A_KMAJOR, B_KMAJOR>(acc, smem_u32(smem_a + stage * kSmemABytes) + wg * (64 * BK * 2),
+                                            smem_u32(smem_b + stage * Cfg::kSmemBBytes), kb == 0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == kStages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+      if (!ok) break;
+      if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+
+      // epilogue: the arithmetic and the rounding points of k_gemm_bf16
+#pragma unroll
+      for (int c0 = 0; c0 < BN; c0 += 64) {  // unrolled: acc must only ever be indexed statically
+        float* v = acc + c0 / 2;  // this thread's 32 values of columns [c0, c0 + 64)
+        if (p.bias != nullptr) {
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int col = n_blk * BN + c0 + 8 * j + frag_col;
+            if (col < p.N) {  // N % 8 == 0 whenever a bias is passed
+              const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p.bias + col));
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                v[4 * j + 2 * h] += f.x;
+                v[4 * j + 2 * h + 1] += f.y;
+              }
+            }
+          }
+        }
+        if (epi_op != EPI_NONE) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int64_t r = (int64_t)m_blk * BM + row0 + 8 * h;
+            const __nv_bfloat16* arow = p.aux + r * p.ld_aux;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int col = n_blk * BN + c0 + 8 * j + frag_col;
+              float2 f = make_float2(0.f, 0.f);
+              if (r < p.M && col < p.N)
+                f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(arow + col));
+              float x0 = v[4 * j + 2 * h], x1 = v[4 * j + 2 * h + 1];
+              if (epi_op == EPI_ADD) {
+                x0 += f.x;
+                x1 += f.y;
+              } else {
+                // ATen multiplies the bf16-rounded GEMM result: reproduce that rounding
+                x0 = __bfloat162float(__float2bfloat16_rn(x0)) * gelu_tanh_grad(f.x);
+                x1 = __bfloat162float(__float2bfloat16_rn(x1)) * gelu_tanh_grad(f.y);
+              }
+              v[4 * j + 2 * h] = x0;
+              v[4 * j + 2 * h + 1] = x1;
+            }
+          }
+        }
+        // the staging buffer we are about to overwrite must have been read by its TMA store
+        if (issuer) tma_store_wait_read<1>();
+        wg_bar_sync(wg);
+        uint8_t* buf = epi + ebuf * kGemm2EpiBufBytes;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = frag_row + 8 * h;
+          uint8_t* rowp = buf + row * 128 + frag_col * 2;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            __nv_bfloat162 o = __floats2bfloat162_rn(v[4 * j + 2 * h], v[4 * j + 2 * h + 1]);
+            // 128-byte swizzle: 16-byte chunk j of row r lives at chunk (j ^ (r & 7))
+            *reinterpret_cast<__nv_bfloat162*>(rowp + ((j ^ (row & 7)) << 4)) = o;
+          }
+        }
+        fence_proxy_async();
+        wg_bar_sync(wg);
+        if (issuer) {
+          tma_store_2d(&tmap_c, buf, n_blk * BN + c0, m_blk * BM + wg * 64);
+          tma_store_commit();
+        }
+        ebuf ^= 1;
+      }
+    }
+    if (issuer) tma_store_wait_all();
+  }
+  if (!ok) asm volatile("trap;");  // a protocol bug becomes a launch error, not a hung GPU
+}
+
 // ---- deferred reduce-scatter: reduce the receive slots of many pushed GEMMs in one launch -----------
 constexpr int kRsMaxItems = 160;
 constexpr int kRsFinishThreads = 256;
@@ -1273,6 +1495,21 @@ static int dispatch_gemm(int bn, bool a_k, bool b_k, const CUtensorMap& ta, cons
   }
 }
 
+template <bool AK, bool BK_>
+static int launch_gemm2(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tc,
+                        const GemmParams& p, int grid, cudaStream_t st) {
+  using Cfg = TileCfg<256>;
+  static bool configured = false;
+  auto kern = k_gemm2_bf16<AK, BK_>;
+  if (!configured) {
+    EDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    configured = true;
+  }
+  kern<<<grid, kGemm2Threads, Cfg::kSmemBytes, st>>>(ta, tb, tc, p);
+  count_launch();
+  return cuda_check(cudaGetLastError(), "k_gemm2_bf16 launch");
+}
+
 static int pick_bn(int64_t N) {
   // 256-wide tiles halve the A traffic per MMA (see TileCfg); 128 only where N leaves nothing
   // for the second half of a 256-wide tile
@@ -1423,15 +1660,11 @@ static int gemm_plain_impl(void* C, const void* A, const void* B, const void* bi
   if (rc) return rc;
   const int sms = sm_count_now();
   int bn = pick_bn(N);
-  if (rt().gemm_force_bn == 128 || rt().gemm_force_bn == 256) bn = (int)rt().gemm_force_bn;
+  const bool forced_bn = rt().gemm_force_bn == 128 || rt().gemm_force_bn == 256;
+  if (forced_bn) bn = (int)rt().gemm_force_bn;
   CUtensorMap ta, tb, tc;
   if (a_kmajor) rc = make_tmap(&ta, A, K, M, lda, BK, BM);
   else rc = make_tmap(&ta, A, M, K, lda, 64, BK);
-  if (rc) return rc;
-  if (b_kmajor) rc = make_tmap(&tb, B, K, N, ldb, BK, bn);
-  else rc = make_tmap(&tb, B, N, K, ldb, 64, BK);
-  if (rc) return rc;
-  rc = make_tmap(&tc, C, N, push ? push->rows_per : M, ldc, 64, BM);
   if (rc) return rc;
   GemmParams p;
   p.C = static_cast<__nv_bfloat16*>(C);
@@ -1515,8 +1748,25 @@ static int gemm_plain_impl(void* C, const void* A, const void* B, const void* bi
       }
     }
   }
+  // a launch that is nothing but a 128 x 256-tile GEMM runs k_gemm2_bf16.  What that kernel gains
+  // is in the epilogue, a couple of k-blocks' worth of clocks per tile: past 256 k-blocks there is
+  // under 1 % to win, and the one such GEMM of the GPT-2 step (LM-head dgrad, K = 50257) measured
+  // 14 % slower with it, so those keep k_gemm_bf16 like everything that is not plain.
+  const bool use2 = gemm2_enabled() && !push && fa.pf_ctas == 0 && p.splits == 1 && bn == 256 &&
+                    !forced_bn && k_blocks <= 256;
+  if (b_kmajor) rc = make_tmap(&tb, B, K, N, ldb, BK, bn);
+  else rc = make_tmap(&tb, B, N, K, ldb, 64, BK);
+  if (rc) return rc;
+  rc = make_tmap(&tc, C, N, push ? push->rows_per : M, ldc, 64, use2 ? 64 : BM);
+  if (rc) return rc;
   const int tiles = units * p.splits;
   int grid = tiles < sms_gemm ? tiles : sms_gemm;
+  if (use2) {
+    if (a_kmajor) return b_kmajor ? launch_gemm2<true, true>(ta, tb, tc, p, grid, st)
+                                  : launch_gemm2<true, false>(ta, tb, tc, p, grid, st);
+    return b_kmajor ? launch_gemm2<false, true>(ta, tb, tc, p, grid, st)
+                    : launch_gemm2<false, false>(ta, tb, tc, p, grid, st);
+  }
   grid += fa.pf_ctas;
   rc = dispatch_gemm<MODE_PLAIN>(bn, a_kmajor != 0, b_kmajor != 0, ta, tb, tc, p, fa, cm, grid, st);
   if (rc || p.splits == 1) return rc;

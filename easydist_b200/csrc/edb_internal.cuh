@@ -88,9 +88,13 @@ struct Runtime {
   int64_t gemm_force_bn = 0;  // tuning aid: 128 / 256 overrides the tile-width heuristic
   int64_t gemm_splitk = 1;   // 1: split K over idle SMs when the tiles fill at most half of them
   int64_t push_sync = 1;     // how push-GEMM CTAs retire (GemmParams::push_sync); 1 measured == 0
+  // plain 128 x 256-tile GEMMs run k_gemm2_bf16 (1) or k_gemm_bf16 like everything else (0: the A/B
+  // switch); -1 = not set yet: EDB_GEMM2 of the environment, else 1
+  int64_t gemm2 = -1;
 };
 
 Runtime& rt();
+bool gemm2_enabled();  // Runtime::gemm2, resolved
 int set_error(int code, const char* fmt, ...);
 int cuda_check(cudaError_t e, const char* what);
 void count_launch();

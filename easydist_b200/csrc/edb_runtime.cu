@@ -20,6 +20,14 @@ static std::atomic<uint64_t> g_launches{0};
 Runtime& rt() { return g_rt; }
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 
+bool gemm2_enabled() {
+  if (g_rt.gemm2 < 0) {
+    const char* e = getenv("EDB_GEMM2");
+    g_rt.gemm2 = (e && !strcmp(e, "0")) ? 0 : 1;
+  }
+  return g_rt.gemm2 != 0;
+}
+
 int set_error(int code, const char* fmt, ...) {
   va_list ap;
   va_start(ap, fmt);
@@ -240,6 +248,10 @@ int edb_set_option(const char* name, int64_t value) {
   else if (!strcmp(name, "spin_timeout_ms")) r.spin_timeout_ms = value;
   else if (!strcmp(name, "gemm_splitk")) r.gemm_splitk = value;
   else if (!strcmp(name, "gemm_force_bn")) r.gemm_force_bn = value;
+  else if (!strcmp(name, "gemm2")) {
+    if (value != 0 && value != 1) return set_error(EDB_E_INVALID, "edb_set_option: gemm2 must be 0 or 1");
+    r.gemm2 = value;
+  }
   else if (!strcmp(name, "ll_max_bytes")) r.ll_max_bytes = value;
   else if (!strcmp(name, "push_sync")) r.push_sync = value;
   else return set_error(EDB_E_INVALID, "edb_set_option: unknown option '%s'", name);
@@ -254,6 +266,7 @@ int edb_get_option(const char* name, int64_t* out) {
   else if (!strcmp(name, "spin_timeout_ms")) *out = r.spin_timeout_ms;
   else if (!strcmp(name, "gemm_splitk")) *out = r.gemm_splitk;
   else if (!strcmp(name, "gemm_force_bn")) *out = r.gemm_force_bn;
+  else if (!strcmp(name, "gemm2")) *out = gemm2_enabled() ? 1 : 0;
   else if (!strcmp(name, "ll_max_bytes")) *out = r.ll_max_bytes;
   else if (!strcmp(name, "push_sync")) *out = r.push_sync;
   else if (!strcmp(name, "sm_count")) *out = r.sm_count;

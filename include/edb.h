@@ -435,7 +435,8 @@ int edb_multi_scale_(int n, void* const* grads, const int64_t* numels, const voi
 /* ---- options / introspection --------------------------------------------------------------- */
 
 /* integer options: "allreduce_oneshot_bytes", "copy_ctas_per_sm", "comm_ctas", "spin_timeout_ms",
- * "ll_max_bytes", "gemm_force_bn", "gemm_splitk" */
+ * "ll_max_bytes", "gemm_force_bn", "gemm_splitk", "gemm2" (1: plain 128 x 256-tile GEMMs run
+ * k_gemm2_bf16, 0: k_gemm_bf16; starts from EDB_GEMM2 of the environment, default 1) */
 int edb_set_option(const char* name, int64_t value);
 int edb_get_option(const char* name, int64_t* value_out);
 /* number of kernels this library has launched since load (all entry points) */
