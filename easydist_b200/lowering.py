@@ -1021,7 +1021,8 @@ def fuse_cross_entropy(gm):
         nll_loss_backward -> _log_softmax_backward_data -> [_to_copy(lp)]     ==> loss.cross_entropy_bwd
 
     Only the exact chain F.cross_entropy(logits.float(), target) traces to is matched (2-D logits,
-    weight=None, reduction mean/sum, log-softmax saved for nothing but its own backward).
+    fp32 log-softmax, weight=None, reduction mean/sum, log-softmax saved for nothing but its own
+    backward).
     Returns the number of chains rewritten."""
     import operator
     from . import loss
@@ -1052,10 +1053,12 @@ def fuse_cross_entropy(gm):
             continue
         if any(u.target is not operator.getitem for u in fwd.users):
             continue
+        # the kernels return an fp32 loss and compute the gradient in fp32: that is the chain's own
+        # precision only when the log-softmax itself is fp32 (fp32 logits, or behind the fp32 cast);
+        # a bf16 log-softmax yields a bf16 loss and a gradient rounded at every ATen op
         val = ls.meta.get("val")
-        if isinstance(val, torch.Tensor) and (val.dim() != 2 or dim not in (1, -1)):
-            continue
-        if val is None and dim != 1:
+        if not isinstance(val, torch.Tensor) or val.dtype != torch.float32 or val.dim() != 2 \
+                or dim not in (1, -1):
             continue
         # optional precision round trip around the fp32 log-softmax
         x, last = x32, lsb

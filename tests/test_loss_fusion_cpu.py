@@ -82,6 +82,45 @@ def test_other_uses_of_log_softmax_block_the_rewrite():
     assert lowering.fuse_cross_entropy(compiled.graph) == 0
 
 
+def test_bf16_log_softmax_is_left_to_aten():
+    """F.cross_entropy on bf16 logits without .float() runs a bf16 log-softmax and returns a bf16
+    loss; the fp32 kernels would change both the loss dtype and the gradient rounding."""
+    set_device_mesh([0], ["dp"], rank=0)
+
+    class M(torch.nn.Module):
+        def __init__(self):
+            super().__init__()
+            self.l = torch.nn.Linear(16, 50)
+
+        def forward(self, x):
+            return self.l(x)
+
+    def step(x, t, model, opt):
+        out = torch.nn.functional.cross_entropy(model(x), t)
+        out.backward()
+        opt.step()
+        opt.zero_grad(True)
+        return out
+
+    torch.manual_seed(0)
+    m, ref = M().bfloat16(), M().bfloat16()
+    ref.load_state_dict(m.state_dict())
+    opt = torch.optim.SGD(m.parameters(), lr=0.1, momentum=0.9)
+    ref_opt = torch.optim.SGD(ref.parameters(), lr=0.1, momentum=0.9)
+    x, t = torch.randn(64, 16).bfloat16(), torch.randint(0, 50, (64,))
+    compiled = api._compile_dp(step, "ddp", "fake", (x, t, m, opt), {}, ops=gloo_ops, native=False)
+    ls = [n for n in compiled.graph.graph.nodes if n.target == aten._log_softmax.default]
+    assert len(ls) == 1 and ls[0].meta["val"].dtype == torch.bfloat16
+    assert lowering.fuse_cross_entropy(compiled.graph) == 0
+    for _ in range(2):
+        l = compiled(x, t, m, opt)
+        l_ref = step(x, t, ref, ref_opt).detach()
+        assert l.dtype == l_ref.dtype == torch.bfloat16 and torch.equal(l, l_ref), (l, l_ref)
+    got = compiled.named_parameters()
+    for name, p in ref.named_parameters():
+        assert torch.equal(got[name], p.detach()), name
+
+
 @pytest.mark.parametrize("opt_kw,expect", [(dict(momentum=0.9), 1), (dict(momentum=0.9, dampening=0.1), 1),
                                            (dict(momentum=0.9, nesterov=True), 0), (dict(), 0)])
 def test_sgd_momentum_triple_is_fused_and_matches_unfused(opt_kw, expect):
