@@ -398,6 +398,54 @@ def _bucket_small_grads(gm, io, ranks, small, region, ops):
         g.replace_all_uses_with(piece, delete_user_cb=lambda u: u not in own)
 
 
+# ---- FX matching helpers of the graph rewrites ------------------------------------------------------------
+
+
+def _call(nd, *targets):
+    return isinstance(nd, Node) and nd.op == "call_function" and nd.target in targets
+
+
+def _val(nd):
+    """The tensor meta["val"] of node nd, else None."""
+    v = nd.meta.get("val") if isinstance(nd, Node) else None
+    return v if isinstance(v, torch.Tensor) else None
+
+
+def _bin(nd, target):
+    """The two operands of a binary `target` node without kwargs (no alpha), else None."""
+    return tuple(nd.args) if _call(nd, target) and len(nd.args) == 2 and not nd.kwargs else None
+
+
+def _other(pair, x):
+    """The operand in `pair` (a binary node's operands, from _bin) that is not x; None if x is not
+    one of them or pair is None."""
+    if pair is None:
+        return None
+    return pair[1] if pair[0] is x else (pair[0] if pair[1] is x else None)
+
+
+def _only_user(nd):
+    return next(iter(nd.users)) if len(nd.users) == 1 else None
+
+
+def _cast_of(nd, dtype):
+    """nd == _to_copy(src, dtype=dtype), strided, on any device -> src, else None."""
+    if _call(nd, aten._to_copy.default) and len(nd.args) == 1 and nd.kwargs.get("dtype") == dtype \
+            and set(nd.kwargs) <= {"dtype", "layout", "device"} \
+            and nd.kwargs.get("layout", torch.strided) == torch.strided:
+        return nd.args[0]
+    return None
+
+
+def _erase_dead(graph, nodes):
+    """Erase exactly the replaced chain `nodes`, readers first; each must have no reader left (no
+    graph-wide DCE: userless comm and in-place nodes must stay)."""
+    order = {nd: i for i, nd in enumerate(graph.nodes)}
+    for nd in sorted(set(nodes), key=lambda nd: -order[nd]):
+        assert not nd.users, (nd, list(nd.users))
+        graph.erase_node(nd)
+
+
 def _is_norm2(nd):
     return _call(nd, aten.linalg_vector_norm.default) and len(nd.args) == 2 and not nd.kwargs \
         and nd.args[1] == 2
@@ -1024,7 +1072,6 @@ def fuse_cross_entropy(gm):
     fp32 log-softmax, weight=None, reduction mean/sum, log-softmax saved for nothing but its own
     backward).
     Returns the number of chains rewritten."""
-    import operator
     from . import loss
     graph = gm.graph
     n = 0
@@ -1056,22 +1103,17 @@ def fuse_cross_entropy(gm):
         # the kernels return an fp32 loss and compute the gradient in fp32: that is the chain's own
         # precision only when the log-softmax itself is fp32 (fp32 logits, or behind the fp32 cast);
         # a bf16 log-softmax yields a bf16 loss and a gradient rounded at every ATen op
-        val = ls.meta.get("val")
-        if not isinstance(val, torch.Tensor) or val.dtype != torch.float32 or val.dim() != 2 \
-                or dim not in (1, -1):
+        val = _val(ls)
+        if val is None or val.dtype != torch.float32 or val.dim() != 2 or dim not in (1, -1):
             continue
         # optional precision round trip around the fp32 log-softmax
         x, last = x32, lsb
-        if x32.op == "call_function" and x32.target == aten._to_copy.default and len(x32.users) == 1 \
-                and x32.kwargs.get("dtype") == torch.float32 and len(lsb.users) == 1:
+        src = _cast_of(x32, torch.float32)
+        if src is not None and set(x32.kwargs) <= {"dtype"} and len(x32.users) == 1 \
+                and len(lsb.users) == 1 and _val(src) is not None:
             cast_back = next(iter(lsb.users))
-            src_val = x32.args[0].meta.get("val") if isinstance(x32.args[0], Node) else None
-            if cast_back.target == aten._to_copy.default and isinstance(src_val, torch.Tensor) \
-                    and cast_back.kwargs.get("dtype") == src_val.dtype \
-                    and set(cast_back.kwargs) <= {"dtype", "layout", "device"} \
-                    and cast_back.kwargs.get("layout", torch.strided) == torch.strided \
-                    and set(x32.kwargs) <= {"dtype"}:
-                x, last = x32.args[0], cast_back
+            if _cast_of(cast_back, _val(src).dtype) is not None:
+                x, last = src, cast_back
         with graph.inserting_before(fwd):
             ce = graph.call_function(loss.cross_entropy_fwd, (x, tgt, ign, red))
             outs = [graph.call_function(operator.getitem, (ce, i)) for i in range(3)]
@@ -1083,57 +1125,17 @@ def fuse_cross_entropy(gm):
                                      (gout, x, tgt, outs[2], outs[1], ign, red))
         dx.meta = dict(last.meta)
         last.replace_all_uses_with(dx)
-        # erase exactly the replaced chain (no graph-wide DCE: userless comm/in-place nodes must stay)
-        dead = [last] if last is not lsb else []
-        dead += [lsb, bwd] + list(fwd.users) + [fwd, ls]
-        if x32 is not x:
-            dead.append(x32)
-        for d in dead:
-            assert not d.users, (d, list(d.users))
-            graph.erase_node(d)
+        _erase_dead(graph, [last, lsb, bwd, *fwd.users, fwd, ls] + ([x32] if x32 is not x else []))
         n += 1
     if n:
         gm.recompile()
     return n
 
 
-def _call(nd, *targets):
-    return isinstance(nd, Node) and nd.op == "call_function" and nd.target in targets
-
-
-def _mul_other(mul, x):
-    """The operand of the binary aten.mul.Tensor node `mul` that is not `x` (None if x is not one)."""
-    if not _call(mul, aten.mul.Tensor) or len(mul.args) != 2 or mul.kwargs:
-        return None
-    a, b = mul.args
-    return b if a is x else (a if b is x else None)
-
-
-def _only_user(nd):
-    return next(iter(nd.users)) if len(nd.users) == 1 else None
-
-
 def _match_rms_chain(r):
     """The decomposed RMSNorm around rsqrt node `r` (workloads.RMSNorm and its autograd backward,
     with or without the fp32 round trip) -> dict of its parts, or None.  Every intermediate must have
     exactly the users the chain gives it."""
-    def val(nd):
-        return nd.meta.get("val") if isinstance(nd, Node) else None
-
-    def f32_copy_of(nd):
-        if _call(nd, aten._to_copy.default) and len(nd.args) == 1 \
-                and nd.kwargs.get("dtype") == torch.float32 \
-                and set(nd.kwargs) <= {"dtype", "layout", "device"}:
-            return nd.args[0]
-        return None
-
-    def cast_to(nd, dtype):
-        """nd == _to_copy(src, dtype) -> src."""
-        if _call(nd, aten._to_copy.default) and len(nd.args) == 1 and nd.kwargs.get("dtype") == dtype \
-                and set(nd.kwargs) <= {"dtype", "layout", "device"}:
-            return nd.args[0]
-        return None
-
     add = r.args[0] if len(r.args) == 1 and not r.kwargs else None
     if not (_call(add, aten.add.Tensor) and len(add.users) == 1 and len(add.args) == 2
             and isinstance(add.args[1], (int, float)) and not add.kwargs):
@@ -1146,12 +1148,12 @@ def _match_rms_chain(r):
     if not (_call(pw2, aten.pow.Tensor_Scalar) and pw2.args[1] == 2 and len(pw2.users) == 1):
         return None
     xa = pw2.args[0]
-    x = f32_copy_of(xa)
+    x = _cast_of(xa, torch.float32)
     cast = x is not None
     if not cast:
         x = xa
-    xv = val(x)
-    if not isinstance(xv, torch.Tensor) or xv.dim() < 2 or (xv.dtype == torch.float32) == cast:
+    xv = _val(x)
+    if xv is None or xv.dim() < 2 or (xv.dtype == torch.float32) == cast:
         return None
     nd_, H = xv.dim(), int(xv.shape[-1])
     last = [[-1], [nd_ - 1]]
@@ -1159,35 +1161,36 @@ def _match_rms_chain(r):
         return None
 
     def is_x(nd):  # x itself or (bf16 model) one of its fp32 copies
-        return nd is x if not cast else f32_copy_of(nd) is x
+        return nd is x if not cast else _cast_of(nd, torch.float32) is x
 
     if len(r.users) != 3:
         return None
     n32 = p1 = pw3 = None
     for u in r.users:
+        o = _other(_bin(u, aten.mul.Tensor), r)
         if _call(u, aten.pow.Tensor_Scalar) and u.args[0] is r and u.args[1] == 3:
             pw3 = u
-        elif _mul_other(u, r) is not None and is_x(_mul_other(u, r)):
+        elif o is not None and is_x(o):
             n32 = u
-        elif _mul_other(u, r) is not None:
+        elif o is not None:
             p1 = u
     if n32 is None or p1 is None or pw3 is None or len(pw3.users) != 1:
         return None
     nb = n32
     if cast:
         nb = _only_user(n32)
-        if cast_to(nb, xv.dtype) is not n32:
+        if _cast_of(nb, xv.dtype) is not n32:
             return None
     if len(nb.users) != 2:
         return None
     def shaped(nd, shape):  # graph transforms insert nodes without meta: unknown shapes pass
-        v = val(nd)
+        v = _val(nd)
         return isinstance(nd, Node) and (v is None or tuple(v.shape) == tuple(shape))
 
     # the forward's mul(normed, w) and the backward's mul(dy, normed), whose only reader is the dw sum
     y = dwm = w_f = dy = None
     for u in nb.users:
-        o = _mul_other(u, nb)
+        o = _other(_bin(u, aten.mul.Tensor), nb)
         if _call(_only_user(u), aten.sum.dim_IntList) and shaped(o, xv.shape):
             dwm, dy = u, o
         elif shaped(o, (H,)):
@@ -1199,15 +1202,15 @@ def _match_rms_chain(r):
             and sorted(d % nd_ for d in sm.args[1]) == list(range(nd_ - 1)) and not sm.kwargs):
         return None
     # backward: g = dy*w (-> fp32), p1 = g*rstd, gx = g*x
-    g32 = _mul_other(p1, r)
-    g = f32_copy_of(g32) if cast else g32
+    g32 = _other(_bin(p1, aten.mul.Tensor), r)
+    g = _cast_of(g32, torch.float32) if cast else g32
     if g is None or len(g32.users) != 2 or (cast and len(g.users) != 1):
         return None
-    w_b = _mul_other(g, dy)
+    w_b = _other(_bin(g, aten.mul.Tensor), dy)
     if w_b is None or not shaped(w_b, (H,)):
         return None
     gx = next(u for u in g32.users if u is not p1)
-    if _mul_other(gx, g32) is None or not is_x(_mul_other(gx, g32)) or len(gx.users) != 1:
+    if not is_x(_other(_bin(gx, aten.mul.Tensor), g32)) or len(gx.users) != 1:
         return None
     s = _only_user(gx)
     if not (_call(s, aten.sum.dim_IntList) and len(s.args) == 3 and list(s.args[1]) in last
@@ -1217,7 +1220,8 @@ def _match_rms_chain(r):
     if not (_call(ms, aten.mul.Scalar) and ms.args == (s, -0.5) and len(ms.users) == 1):
         return None
     m5 = _only_user(ms)
-    if _mul_other(m5, ms) is not pw3 or _only_user(pw3) is not m5 or len(m5.users) != 1:
+    if _other(_bin(m5, aten.mul.Tensor), ms) is not pw3 or _only_user(pw3) is not m5 \
+            or len(m5.users) != 1:
         return None
     ex = _only_user(m5)
     if not (_call(ex, aten.expand.default) and list(ex.args[1]) == list(xv.shape)
@@ -1227,7 +1231,7 @@ def _match_rms_chain(r):
     if not (_call(dv, aten.div.Scalar) and dv.args[1] == H and len(dv.users) == 1):
         return None
     p2 = _only_user(dv)
-    q = _mul_other(p2, dv)
+    q = _other(_bin(p2, aten.mul.Tensor), dv)
     if not (_call(q, aten.mul.Scalar) and q.args[1] == 2.0 and len(q.users) == 1):
         return None
     pw1 = q.args[0]
@@ -1239,7 +1243,7 @@ def _match_rms_chain(r):
         if len(p.users) != 1:
             return None
         pc = _only_user(p) if cast else p
-        if cast and cast_to(pc, xv.dtype) is not p:
+        if cast and _cast_of(pc, xv.dtype) is not p:
             return None
         if len(pc.users) != 1:
             return None
@@ -1254,9 +1258,8 @@ def _match_rms_chain(r):
             and _only_user(u1) is u2 and _call(u2, aten.add.Tensor) and len(u2.args) == 2 \
             and not u2.kwargs and set(u2.args) == {u1, p2c}:
         run = u1.args[1] if u1.args[0] is p1c else u1.args[0]
-        rv = val(run)
-        if not isinstance(run, Node) or run in (p1c, p2c) or not isinstance(rv, torch.Tensor) \
-                or tuple(rv.shape) != tuple(xv.shape) or rv.dtype != xv.dtype:
+        rv = _val(run)
+        if rv is None or run in (p1c, p2c) or tuple(rv.shape) != tuple(xv.shape) or rv.dtype != xv.dtype:
             return None
         dx = u2
     else:
@@ -1266,9 +1269,37 @@ def _match_rms_chain(r):
         chain += [nb, g, p1c, p2c]
     if run is not None:
         chain.append(u1)
-    copies = list({xa, _mul_other(n32, r), _mul_other(gx, g32), pw1.args[0]}) if cast else []
+    copies = list({xa, _other(_bin(n32, aten.mul.Tensor), r), _other(_bin(gx, aten.mul.Tensor), g32),
+                   pw1.args[0]}) if cast else []
     return dict(x=x, w_f=w_f, w_b=w_b, dy=dy, eps=eps, y=y, r=r, sm=sm, dx=dx, run=run,
                 chain=chain, x_copies=copies)
+
+
+def _fold_accumulation(graph, target):
+    """Gradient accumulation behind a norm backward node of `target`: add(getitem(bwd, 0), other),
+    with `other` of the same shape and dtype and computed before bwd, becomes bwd(..., _add=other).
+    Returns the number of adds folded."""
+    order = {nd: i for i, nd in enumerate(graph.nodes)}
+    n = 0
+    for nd in list(graph.nodes):
+        pair = _bin(nd, aten.add.Tensor)
+        for g, other in ((pair, pair[::-1]) if pair else ()):
+            if not (_call(g, operator.getitem) and g.args[1] == 0 and len(g.users) == 1
+                    and isinstance(other, Node)):
+                continue
+            bw = g.args[0]
+            if not (_call(bw, target) and "_add" not in bw.kwargs):
+                continue
+            gv, ov = _val(g), _val(other)
+            if gv is None or ov is None or tuple(gv.shape) != tuple(ov.shape) \
+                    or gv.dtype != ov.dtype or order[other] > order[bw]:
+                continue
+            bw.kwargs = dict(bw.kwargs, _add=other)
+            nd.replace_all_uses_with(g)
+            graph.erase_node(nd)
+            n += 1
+            break
+    return n
 
 
 def fuse_rms_norm(gm):
@@ -1282,7 +1313,6 @@ def fuse_rms_norm(gm):
         retargeted to norm.fused_rms_norm(_backward), with a following add(dx, g) folded into `_add`.
     Chains with any extra reader of an intermediate are left alone.  Returns (forward, backward)
     counts."""
-    import operator
     from . import norm
     graph = gm.graph
     n_fwd = n_bwd = 0
@@ -1313,10 +1343,7 @@ def fuse_rms_norm(gm):
         dx2.meta, dwv.meta = dict(m["dx"].meta), dict(m["sm"].meta)
         m["dx"].replace_all_uses_with(dx2)
         m["sm"].replace_all_uses_with(dwv)
-        # erase exactly the replaced chain, readers first
-        for d in sorted(m["chain"], key=lambda nd: -order[nd]):
-            assert not d.users, (d, list(d.users))
-            graph.erase_node(d)
+        _erase_dead(graph, m["chain"])
         for c in m["x_copies"]:
             if not c.users:
                 graph.erase_node(c)
@@ -1330,26 +1357,7 @@ def fuse_rms_norm(gm):
         elif _call(nd, aten._fused_rms_norm_backward.default):
             nd.target = norm.fused_rms_norm_backward
             n_bwd += 1
-    order = {nd: i for i, nd in enumerate(graph.nodes)}
-    for nd in list(graph.nodes):
-        if not _call(nd, aten.add.Tensor) or len(nd.args) != 2 or nd.kwargs:
-            continue
-        for gi, oi in ((0, 1), (1, 0)):
-            g, other = nd.args[gi], nd.args[oi]
-            if not (_call(g, operator.getitem) and g.args[1] == 0 and len(g.users) == 1
-                    and isinstance(other, Node)):
-                continue
-            bw = g.args[0]
-            if not (_call(bw, norm.fused_rms_norm_backward) and "_add" not in bw.kwargs):
-                continue
-            gv, ov = g.meta.get("val"), other.meta.get("val")
-            if gv is None or ov is None or tuple(gv.shape) != tuple(ov.shape) \
-                    or gv.dtype != ov.dtype or order[other] > order[bw]:
-                continue
-            bw.kwargs = dict(bw.kwargs, _add=other)
-            nd.replace_all_uses_with(g)
-            graph.erase_node(nd)
-            break
+    _fold_accumulation(graph, norm.fused_rms_norm_backward)
     if n_fwd or n_bwd:
         graph.lint()
         gm.recompile()
@@ -1361,7 +1369,6 @@ def fuse_swiglu(gm):
     ==> act.swiglu_fwd(a, b) / act.swiglu_bwd(dy, a, b) (edb_rms.cu).  The silu node is erased: no
     [tokens, ffn] tensor besides a and b stays alive from forward to backward.  Only a silu with
     exactly those two readers is rewritten.  Returns (forward, backward) counts."""
-    import operator
     from . import act
     graph = gm.graph
     n = 0
@@ -1372,11 +1379,11 @@ def fuse_swiglu(gm):
         u = list(s.users)
         found = None
         for f, m1 in ((u[0], u[1]), (u[1], u[0])):
-            b, dy = _mul_other(f, s), _mul_other(m1, s)
+            b, dy = _other(_bin(f, aten.mul.Tensor), s), _other(_bin(m1, aten.mul.Tensor), s)
             if b is None or dy is None or b is s or dy is s:
                 continue
             for m2 in b.users:
-                sb = _only_user(m2) if _mul_other(m2, b) is dy else None
+                sb = _only_user(m2) if _other(_bin(m2, aten.mul.Tensor), b) is dy else None
                 if _call(sb, aten.silu_backward.default) and sb.args == (m2, a) and not sb.kwargs:
                     found = (f, m1, m2, sb, b, dy)
                     break
@@ -1397,24 +1404,12 @@ def fuse_swiglu(gm):
         dgate.meta, dup.meta = dict(sb.meta), dict(m1.meta)
         sb.replace_all_uses_with(dgate)
         m1.replace_all_uses_with(dup)
-        for d in (sb, m2, m1, f, s):
-            assert not d.users, (d, list(d.users))
-            graph.erase_node(d)
+        _erase_dead(graph, [sb, m2, m1, f, s])
         n += 1
     if n:
         graph.lint()
         gm.recompile()
     return n, n
-
-
-def _rope_val(nd):
-    v = nd.meta.get("val") if isinstance(nd, Node) else None
-    return v if isinstance(v, torch.Tensor) else None
-
-
-def _bin(nd, target):
-    """The two operands of a binary `target` node without kwargs (no alpha), else None."""
-    return tuple(nd.args) if _call(nd, target) and len(nd.args) == 2 and not nd.kwargs else None
 
 
 def _rope_halves(lo, hi, hd):
@@ -1431,7 +1426,7 @@ def _rope_half(nd):
     if not _call(nd, aten.slice.Tensor) or nd.kwargs or not 4 <= len(nd.args) <= 5:
         return None
     src, dim, lo, hi = nd.args[:4]
-    v = _rope_val(src)
+    v = _val(src)
     if v is None or v.dim() != 4 or dim not in (3, -1) or (len(nd.args) == 5 and nd.args[4] != 1):
         return None
     w = _rope_halves(lo, hi, int(v.shape[-1]))
@@ -1452,7 +1447,7 @@ def _rope_filled(nd):
 
 def _rope_table(nd, x):
     """nd if it is a [T, hd/2] table of x's dtype (x: [B, H, T, hd]), else None."""
-    v, xv = _rope_val(nd), _rope_val(x)
+    v, xv = _val(nd), _val(x)
     if v is None or xv is None or v.dtype != xv.dtype \
             or tuple(v.shape) != (int(xv.shape[2]), int(xv.shape[3]) // 2):
         return None
@@ -1489,11 +1484,6 @@ def _rope_rotated(rc):
     if h2 is None or h1 is None or h2[1] != 1 or h1[1] != 0 or h2[0] is not h1[0]:
         return None
     return h2[0], [ng, ng.args[0], lo]
-
-
-def _other(ops, x):
-    """The operand of a binary node's `ops` that is not x (None if x is not one)."""
-    return ops[1] if ops[0] is x else (ops[0] if ops[1] is x else None)
 
 
 def _match_rope_fwd_split(cat):
@@ -1644,7 +1634,7 @@ def fuse_rope(gm):
             m = _match_rope_fwd_half(nd) or _match_rope_bwd_split(nd) or _match_rope_bwd_half(nd)
         if m is None:
             continue
-        out, chain = m["out"], list(dict.fromkeys(m["chain"]))
+        out, chain = m["out"], list(m["chain"])
         target, kw = out, {}
         if m["inverse"]:
             tr = _only_user(out)
@@ -1654,17 +1644,14 @@ def fuse_rope(gm):
                     and cl.kwargs == {"memory_format": torch.contiguous_format}:
                 target, kw = cl, {"transposed": True}
                 chain += [tr, cl]
-        if not kw and _rope_val(out) is not None:
-            kw = {"stride": list(_rope_val(out).stride())}
+        if not kw and _val(out) is not None:
+            kw = {"stride": list(_val(out).stride())}
         with graph.inserting_before(out):
             new = graph.call_function(rope.rope, (m["x"], m["c"], m["s"], m["inverse"]), kw)
         new.meta = dict(target.meta)
         target.replace_all_uses_with(new)
-        order = {n: i for i, n in enumerate(graph.nodes)}
-        for d in sorted(chain, key=lambda n: -order[n]):
-            assert not d.users, (d, list(d.users))
-            graph.erase_node(d)
-            gone.add(d)
+        _erase_dead(graph, chain)
+        gone.update(chain)
         for t in dict.fromkeys(m.get("dead", ())):
             if not t.users:
                 graph.erase_node(t)
@@ -1741,13 +1728,18 @@ _ALIAS_OPS = (aten.t.default, aten.view.default, aten._unsafe_view.default, aten
               aten.permute.default, aten.alias.default, aten.detach.default, aten.slice.Tensor,
               aten.select.int, aten.flatten.using_ints, aten.reshape.default, aten.expand.default,
               aten.unsqueeze.default, aten.squeeze.dim, aten.as_strided.default)
+# the views a side-stream GEMM result may pass through before its join (parallel_wgrad_gemms): they
+# only relabel shape and strides; every other reader, a reshape (which may copy) included, waits
+_VIEW_ONLY = (aten.t.default, aten.view.default, aten._unsafe_view.default, aten.transpose.int,
+              aten.permute.default, aten.alias.default, aten.detach.default, aten.unsqueeze.default,
+              aten.squeeze.dim)
 
 
-def _memory_readers(x):
-    """Every non-view node that reads memory of `x`: through x, the views x was taken from, and any
-    view of those."""
+def _memory_readers(x, through=_ALIAS_OPS):
+    """Every node that reads memory of `x` other than through one of the ops `through`: through x,
+    the views x was taken from, and any view of those."""
     root = x
-    while _call(root, *_ALIAS_OPS):
+    while _call(root, *through):
         root = root.args[0]
     readers, frontier, seen = [], [root], {root}
     while frontier:
@@ -1756,7 +1748,7 @@ def _memory_readers(x):
             if u in seen:
                 continue
             seen.add(u)
-            if _call(u, *_ALIAS_OPS) and u.args[0] is nd:
+            if _call(u, *through) and u.args[0] is nd:
                 frontier.append(u)
             else:
                 readers.append(u)
@@ -1771,11 +1763,10 @@ def _fold_clip_scale(gm, clamp):
     left alone.  -> number of mul_ nodes replaced."""
     from . import clip, optim
     graph = gm.graph
-    dt = clamp.meta["val"].dtype if isinstance(clamp.meta.get("val"), torch.Tensor) else None
+    dt = _val(clamp).dtype if _val(clamp) is not None else None
     muls = [u for u in clamp.users if _call(u, aten.mul_.Tensor) and len(u.args) == 2
             and u.args[1] is clamp and u.args[0] is not clamp and not u.kwargs
-            and isinstance(u.args[0].meta.get("val"), torch.Tensor)
-            and u.args[0].meta["val"].dtype == dt]
+            and _val(u.args[0]) is not None and _val(u.args[0]).dtype == dt]
     if not muls or len({m.args[0] for m in muls}) != len(muls):
         return 0
     pos = {nd: i for i, nd in enumerate(graph.nodes)}
@@ -1821,9 +1812,9 @@ def fuse_grad_clip(gm):
     n_norm = n_scale = 0
     for ch in _match_clip(gm):
         norms, stack = ch["norms"], ch["stack"]
-        dts = {nd.meta["val"].dtype for nd in norms if isinstance(nd.meta.get("val"), torch.Tensor)}
-        if len(dts) != 1 or any(not isinstance(nd.args[0].meta.get("val"), torch.Tensor)
-                                or nd.args[0].meta["val"].dtype not in dts for nd in norms):
+        dts = {_val(nd).dtype for nd in norms if _val(nd) is not None}
+        if len(dts) != 1 or any(_val(nd.args[0]) is None or _val(nd.args[0]).dtype not in dts
+                                for nd in norms):
             continue
         with graph.inserting_before(stack):
             gn = graph.call_function(clip.grad_norms, ([nd.args[0] for nd in norms],))
@@ -1843,9 +1834,6 @@ def fuse_grad_clip(gm):
     return n_norm, n_scale
 
 
-_VIEW_ONLY = None
-
-
 def parallel_wgrad_gemms(gm):
     """Opt-in (`EDB_GEMM_SIDE=1`): GEMMs whose result is first *computed on* much later (weight
     gradients: read by the optimizer) are launched on a second compute stream and joined right in
@@ -1853,12 +1841,7 @@ def parallel_wgrad_gemms(gm):
     which fills the wave a 128-tile GEMM leaves 14 % empty, and hides launch gaps.  Only metadata
     ops (t / view / permute ...) may touch the result before the join.  Returns the number of GEMMs
     moved."""
-    global _VIEW_ONLY
     from . import gemm
-    if _VIEW_ONLY is None:
-        _VIEW_ONLY = {aten.t.default, aten.view.default, aten._unsafe_view.default,
-                      aten.transpose.int, aten.permute.default, aten.alias.default,
-                      aten.detach.default, aten.unsqueeze.default, aten.squeeze.dim}
     graph = gm.graph
     nodes = list(graph.nodes)
     order = {n: i for i, n in enumerate(nodes)}
@@ -1868,17 +1851,7 @@ def parallel_wgrad_gemms(gm):
     for node in reversed(nodes):
         if node.op != "call_function" or node.target is not gemm.mm or node.kwargs:
             continue
-        consumers, frontier, seen = [], [node], {node}
-        while frontier:
-            cur = frontier.pop()
-            for u in cur.users:
-                if u in seen:
-                    continue
-                seen.add(u)
-                if u.op == "call_function" and u.target in _VIEW_ONLY:
-                    frontier.append(u)
-                else:
-                    consumers.append(u)
+        consumers = _memory_readers(node, _VIEW_ONLY)
         if not consumers:
             continue
         first = min(consumers, key=lambda u: order[u])
@@ -1905,25 +1878,38 @@ def fuse_gemm_epilogues(gm):
     when the GEMM result has no other reader and the second operand is a bf16 matrix of the
     result's shape (2-D, or a view of one: the traced Linear works on [tokens, features]).  The
     reference runs these as separate ATen kernels (a14: op-by-op FX execution)."""
-    from . import gemm
+    from . import gemm, norm
     graph = gm.graph
     n = 0
     bf16 = torch.bfloat16
 
-    def val(nd):
-        return nd.meta.get("val") if isinstance(nd, Node) else None
-
     def gemm_behind(nd):
         """nd == gemm.mm/addmm(...), or a shape-only view of it with a single reader chain."""
         chain = []
-        while isinstance(nd, Node) and nd.op == "call_function" and \
-                nd.target in (aten.view.default, aten._unsafe_view.default) and len(nd.users) == 1:
+        while _call(nd, aten.view.default, aten._unsafe_view.default) and len(nd.users) == 1:
             chain.append(nd)
             nd = nd.args[0]
-        if isinstance(nd, Node) and nd.op == "call_function" and nd.target in (gemm.mm, gemm.addmm) \
-                and len(nd.users) == 1 and not nd.kwargs.get("_side"):
+        if _call(nd, gemm.mm, gemm.addmm) and len(nd.users) == 1 and not nd.kwargs.get("_side"):
             return nd, chain
         return None, chain
+
+    def fuse(node, g, chain, target, operand, *extra):
+        """node == elementwise(g behind the views `chain`, operand) -> target(a, b, operand viewed
+        2-D, *extra) in g's place, viewed back to node's shape."""
+        gv, ov, nv = _val(g), _val(operand), _val(node)
+        with graph.inserting_before(g):
+            op2d = operand if ov.dim() == 2 else graph.call_function(
+                aten.view.default, args=(operand, list(gv.shape)))
+            a, b = g.args[-2:]
+            fused = graph.call_function(target, args=(a, b, op2d, *extra),
+                                        kwargs={k: v for k, v in g.kwargs.items() if k == "_pf"})
+            fused.meta = dict(g.meta)
+            out = fused
+            if nv.dim() != 2:
+                out = graph.call_function(aten.view.default, args=(fused, list(nv.shape)))
+                out.meta = dict(node.meta)
+        node.replace_all_uses_with(out)
+        _erase_dead(graph, [node, *chain, g])
 
     for node in list(graph.nodes):
         if node.op != "call_function":
@@ -1932,8 +1918,8 @@ def fuse_gemm_epilogues(gm):
             for gi, oi in ((1, 0), (0, 1)):
                 g, chain = gemm_behind(node.args[gi])
                 other = node.args[oi]
-                gv, ov, nv = val(g), val(other), val(node)
-                if g is None or not isinstance(other, Node) or gv is None or ov is None or nv is None:
+                gv, ov, nv = _val(g), _val(other), _val(node)
+                if gv is None or ov is None or nv is None:
                     continue
                 if ov.dtype != bf16 or gv.dtype != bf16 or gv.shape[1] % 8 or \
                         tuple(ov.shape) != tuple(nv.shape) or ov.numel() != gv.numel():
@@ -1943,31 +1929,13 @@ def fuse_gemm_epilogues(gm):
                 order = {nd: i for i, nd in enumerate(graph.nodes)}
                 if order[other] > order[g]:
                     continue  # the residual must exist when the GEMM runs
-                with graph.inserting_before(g):
-                    res2d = other if ov.dim() == 2 else graph.call_function(
-                        aten.view.default, args=(other, list(gv.shape)))
-                    if g.target is gemm.addmm:
-                        bias, a, b = g.args
-                    else:
-                        (a, b), bias = g.args, None
-                    fused = graph.call_function(gemm.mm_add, args=(a, b, res2d, bias),
-                                                kwargs={k: v for k, v in g.kwargs.items() if k == "_pf"})
-                    fused.meta = dict(g.meta)
-                    out = fused
-                    if nv.dim() != 2:
-                        out = graph.call_function(aten.view.default, args=(fused, list(nv.shape)))
-                        out.meta = dict(node.meta)
-                node.replace_all_uses_with(out)
-                graph.erase_node(node)
-                for c in chain:
-                    graph.erase_node(c)
-                graph.erase_node(g)
+                fuse(node, g, chain, gemm.mm_add, other, g.args[0] if g.target is gemm.addmm else None)
                 n += 1
                 break
         elif node.target == aten.gelu_backward.default and node.kwargs.get("approximate") == "tanh":
             g, chain = gemm_behind(node.args[0])
             pre = node.args[1]
-            gv, pv, nv = val(g), val(pre), val(node)
+            gv, pv, nv = _val(g), _val(pre), _val(node)
             if g is None or g.target is not gemm.mm or gv is None or pv is None or nv is None:
                 continue
             if pv.dtype != bf16 or gv.dtype != bf16 or gv.shape[1] % 8 or pv.numel() != gv.numel() \
@@ -1976,48 +1944,9 @@ def fuse_gemm_epilogues(gm):
             order = {nd: i for i, nd in enumerate(graph.nodes)}
             if order[pre] > order[g]:
                 continue
-            with graph.inserting_before(g):
-                pre2d = pre if pv.dim() == 2 else graph.call_function(
-                    aten.view.default, args=(pre, list(gv.shape)))
-                a, b = g.args
-                fused = graph.call_function(gemm.mm_gelu_bwd, args=(a, b, pre2d),
-                                            kwargs={k: v for k, v in g.kwargs.items() if k == "_pf"})
-                fused.meta = dict(g.meta)
-                out = fused
-                if nv.dim() != 2:
-                    out = graph.call_function(aten.view.default, args=(fused, list(nv.shape)))
-                    out.meta = dict(node.meta)
-            node.replace_all_uses_with(out)
-            graph.erase_node(node)
-            for c in chain:
-                graph.erase_node(c)
-            graph.erase_node(g)
+            fuse(node, g, chain, gemm.mm_gelu_bwd, pre)
             n += 1
-    # gradient accumulation behind a LayerNorm backward: add(getitem(ln_bwd, 0), other) -> _add=other
-    from . import norm
-    order = {nd: i for i, nd in enumerate(graph.nodes)}
-    for node in list(graph.nodes):
-        if node.op != "call_function" or node.target != aten.add.Tensor or len(node.args) != 2 \
-                or node.kwargs:
-            continue
-        for gi, oi in ((0, 1), (1, 0)):
-            g, other = node.args[gi], node.args[oi]
-            if not (isinstance(g, Node) and g.op == "call_function" and g.target is operator.getitem
-                    and g.args[1] == 0 and len(g.users) == 1 and isinstance(other, Node)):
-                continue
-            ln = g.args[0]
-            if not (isinstance(ln, Node) and ln.target is norm.native_layer_norm_backward
-                    and "_add" not in ln.kwargs):
-                continue
-            lv, ov = val(g), val(other)
-            if lv is None or ov is None or tuple(lv.shape) != tuple(ov.shape) or lv.dtype != ov.dtype \
-                    or order[other] > order[ln]:
-                continue
-            ln.kwargs = dict(ln.kwargs, _add=other)
-            node.replace_all_uses_with(g)
-            graph.erase_node(node)
-            n += 1
-            break
+    n += _fold_accumulation(graph, norm.native_layer_norm_backward)
     if n:
         graph.lint()
         gm.recompile()
@@ -2029,7 +1958,6 @@ def dispatch_compute(gm, counts=None):
     `counts` (a dict), when given, receives the (forward, backward) counts of the RMSNorm, SwiGLU and
     RoPE rewrites as "rms_norm", "swiglu" and "rope", and the (norm, scale) counts of the gradient
     clipping rewrite as "clip"."""
-    import os
     from . import gemm, norm
     native_ln = os.environ.get("EDB_NATIVE_LN", "1") == "1"
     counts = {} if counts is None else counts
@@ -2048,24 +1976,19 @@ def dispatch_compute(gm, counts=None):
     for node in gm.graph.nodes:
         if node.op != "call_function":
             continue
-        if not native_ln:
-            pass
-        elif node.target == aten.native_layer_norm.default:
+        val = _val(node)
+        if native_ln and node.target == aten.native_layer_norm.default:
             node.target = norm.native_layer_norm
             n += 1
-            continue
-        elif node.target == aten.native_layer_norm_backward.default:
+        elif native_ln and node.target == aten.native_layer_norm_backward.default:
             node.target = norm.native_layer_norm_backward
             n += 1
-            continue
-        if native_ln and node.target == aten.sum.dim_IntList:
+        elif native_ln and node.target == aten.sum.dim_IntList:
             node.target = norm.sum_dim_intlist
             n += 1
+        elif val is None or val.dtype != torch.bfloat16:
             continue
-        val = node.meta.get("val")
-        if not isinstance(val, torch.Tensor) or val.dtype != torch.bfloat16:
-            continue
-        if node.target == aten.mm.default:
+        elif node.target == aten.mm.default:
             node.target = gemm.mm
             if "edb_pf" in node.meta:
                 node.kwargs = {"_pf": node.meta["edb_pf"]}
