@@ -98,6 +98,8 @@ def _prepare(t, unit_dim):
     else:
         return None
     ld = rowmajor.stride(0)
+    if ld < rowmajor.shape[1]:
+        return None  # rows overlap (an expanded operand has ld 0): not a matrix TMA can describe
     if ld % 8 or rowmajor.data_ptr() % 16:
         rowmajor = _padded_copy(rowmajor)
         ld = rowmajor.stride(0)
@@ -190,7 +192,7 @@ def _launch(a, b, bias, side=0, pf=None, epi=None):
     if epi is not None:
         op, aux = epi
         if N % 8 or aux.dtype != torch.bfloat16 or aux.shape != (M, N) or aux.stride(1) != 1 or \
-                aux.stride(0) % 8 or aux.data_ptr() % 16:
+                aux.stride(0) % 8 or aux.stride(0) < N or aux.data_ptr() % 16:
             return None
     with _SideStream(side) as fork:
         if epi is not None:

@@ -1953,6 +1953,22 @@ def fuse_gemm_epilogues(gm):
     return n
 
 
+def _reshape_views_of(node):
+    """gemm.mm returns an output whose N is not a multiple of 8 as a narrowed view of a padded
+    buffer (row stride round_up(N, 8)), where the graph was traced on a contiguous one.  The
+    `view` / `_unsafe_view` nodes reached from `node` through view ops become `reshape`, which
+    returns the same view wherever the strides allow it and copies only where a view would raise
+    (e.g. flattening [M, N] to [M * N])."""
+    frontier = [node]
+    while frontier:
+        nd = frontier.pop()
+        for u in nd.users:
+            if _call(u, *_ALIAS_OPS) and u.args[0] is nd:
+                if u.target in (aten.view.default, aten._unsafe_view.default):
+                    u.target = aten.reshape.default
+                frontier.append(u)
+
+
 def dispatch_compute(gm, counts=None):
     """Route bf16 `aten.mm` / `aten.addmm` nodes to the wgmma GEMM (sharded-op kernel dispatch).
     `counts` (a dict), when given, receives the (forward, backward) counts of the RMSNorm, SwiGLU and
@@ -1992,6 +2008,8 @@ def dispatch_compute(gm, counts=None):
             node.target = gemm.mm
             if "edb_pf" in node.meta:
                 node.kwargs = {"_pf": node.meta["edb_pf"]}
+            if val.dim() == 2 and val.shape[1] % 8:
+                _reshape_views_of(node)
             n += 1
         elif node.target == aten.addmm.default and not node.kwargs:
             node.target = gemm.addmm

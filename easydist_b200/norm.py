@@ -39,12 +39,22 @@ def _stream(t):
     return torch.cuda.current_stream(t.device).cuda_stream
 
 
+def _dense(t):
+    """`t` when it is contiguous and 16-byte aligned, the layout every LayerNorm and RMSNorm kernel
+    reads (H consecutive elements per row, 16-byte vectors); otherwise a dense copy in a fresh
+    allocation.  `.contiguous()` alone keeps a contiguous view at a misaligned storage offset."""
+    if t.is_contiguous() and t.data_ptr() % 16 == 0:
+        return t
+    return t.clone(memory_format=torch.contiguous_format)
+
+
 def native_layer_norm(input, normalized_shape, weight, bias, eps):
     if not _supported(input, normalized_shape, weight) or (bias is not None and bias.dtype != input.dtype):
         if not isinstance(input, FakeTensor):
             _stats["aten_ln"] += 1
         return aten.native_layer_norm.default(input, normalized_shape, weight, bias, eps)
-    x = input.contiguous()
+    x, weight = _dense(input), _dense(weight)
+    bias = _dense(bias) if bias is not None else None
     H = int(normalized_shape[0])
     rows = x.numel() // H
     y = torch.empty_like(x)
@@ -86,8 +96,7 @@ def native_layer_norm_backward(grad_out, input, normalized_shape, mean, rstd, we
         if _add is not None:
             res = (aten.add.Tensor(res[0], _add),) + tuple(res[1:])
         return res
-    x = input.contiguous()
-    dy = grad_out.contiguous()
+    x, dy, weight = _dense(input), _dense(grad_out), _dense(weight)
     H = int(normalized_shape[0])
     rows = x.numel() // H
     dx = torch.empty_like(x)
@@ -95,7 +104,7 @@ def native_layer_norm_backward(grad_out, input, normalized_shape, mean, rstd, we
     db = torch.empty_like(weight) if output_mask[2] else None
     ws = _workspace(H, x.device)
     lib = _lib.load()
-    add = _add.contiguous() if _add is not None else None
+    add = _dense(_add) if _add is not None else None
     check(lib.edb_layer_norm_bwd_add(dx.data_ptr(), dw.data_ptr() if dw is not None else None,
                                      db.data_ptr() if db is not None else None, dy.data_ptr(),
                                      x.data_ptr(), mean.contiguous().data_ptr(),
@@ -152,7 +161,7 @@ def _rms_supported(x, w, H):
     if w is None or w.dtype != x.dtype or tuple(w.shape) != (H,) or x.shape[-1] != H:
         return False
     epv = 8 if x.dtype == torch.bfloat16 else 4
-    return H % epv == 0 and H <= RMS_MAX_H and w.is_contiguous() and w.data_ptr() % 16 == 0
+    return H % epv == 0 and H <= RMS_MAX_H
 
 
 def _rms_fwd_chain(x, w, eps):
@@ -204,7 +213,7 @@ def rms_norm_fwd(x, w, eps, mode):
         if mode == RMS_FUSED:
             return aten._fused_rms_norm.default(x, [H], w, eps)
         return _rms_fwd_chain(x, w, eps)
-    x = x.contiguous()
+    x, w = _dense(x), _dense(w)
     rows = x.numel() // H
     y = torch.empty_like(x)
     rstd = torch.empty(list(x.shape[:-1]) + [1], dtype=torch.float32, device=x.device)
@@ -232,8 +241,7 @@ def rms_norm_bwd(dy, x, rstd, w, mode, output_mask, *, _add=None):
                 dx = aten.add.Tensor(dx, _add)
             return dx, dw
         return _rms_bwd_chain(dy, x, rstd, w, output_mask, _add)
-    x = x.contiguous()
-    dy = dy.contiguous()
+    x, dy, w = _dense(x), _dense(dy), _dense(w)
     rows = x.numel() // H
     dx = torch.empty_like(x)
     dw = torch.empty_like(w) if output_mask[1] else None
@@ -245,7 +253,7 @@ def rms_norm_bwd(dy, x, rstd, w, mode, output_mask, *, _add=None):
         check(lib.edb_rms_norm_bwd_workspace(H, byref(nbytes)))
         ws = _rms_workspaces[key] = torch.empty(max(16, nbytes.value), dtype=torch.uint8,
                                                 device=x.device)
-    add = _add.contiguous() if _add is not None else None
+    add = _dense(_add) if _add is not None else None
     check(lib.edb_rms_norm_bwd(dx.data_ptr(), dw.data_ptr() if dw is not None else None,
                                dy.data_ptr(), x.data_ptr(), rstd.contiguous().data_ptr(), w.data_ptr(),
                                add.data_ptr() if add is not None else None, ws.data_ptr(), rows, H,
