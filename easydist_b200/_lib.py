@@ -115,6 +115,11 @@ SIGNATURES = {
                          _I64P, _I64P, c_int64, c_int, c_int, c_void_p]),
     "edb_swiglu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
                                c_void_p]),
+    "edb_embedding_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
+                                  c_int64, c_int64, c_int64, c_int, c_int, c_void_p]),
+    "edb_embedding_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int64,
+                                  c_int64, c_int64, c_int64, c_int, c_int, c_int, c_void_p]),
+    "edb_embedding_bwd_workspace": (c_int, [c_int64, c_int64, POINTER(c_size_t)]),
     "edb_colsum": (c_int,[c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int, c_void_p]),
     "edb_colsum_workspace": (c_int, [c_int64, POINTER(c_size_t)]),
     "edb_cross_entropy_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,

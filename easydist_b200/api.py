@@ -182,6 +182,7 @@ def _finish(gm, params, buffers, named_states, args, kwargs, ops, native, io=Non
         info["swiglu_nodes"] = counts["swiglu"]
         info["rope_nodes"] = counts["rope"]
         info["clip_nodes"] = counts["clip"]
+        info["embed_nodes"] = counts["embed"]
         if ranks is not None and len(ranks) > 1 and (push or info.get("fused")):
             # static race check of the lowered graph against the epoch-protocol contract (diagnostic:
             # problems are logged and reported in `info`; EDB_VERIFY_STRICT=1 makes them fatal)

@@ -18,7 +18,7 @@ LIB_PATH = os.path.join(HERE, "libedb.so")
 BUILD_DIR = os.path.join(HERE, "csrc", "_build")
 
 HEADERS = ["edb_internal.cuh", "edb_vec.cuh"]
-SOURCES = ["edb_runtime.cu", "edb_reshard.cu", "edb_ll.cu", "edb_norm.cu", "edb_rms.cu", "edb_rope.cu", "edb_loss.cu", "edb_optim.cu", "edb_clip.cu", "edb_gemm.cu"]
+SOURCES = ["edb_runtime.cu", "edb_reshard.cu", "edb_ll.cu", "edb_norm.cu", "edb_rms.cu", "edb_rope.cu", "edb_embed.cu", "edb_loss.cu", "edb_optim.cu", "edb_clip.cu", "edb_gemm.cu"]
 
 ARCH = "arch=compute_90a,code=sm_90a"
 

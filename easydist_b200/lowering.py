@@ -1834,6 +1834,92 @@ def fuse_grad_clip(gm):
     return n_norm, n_scale
 
 
+def _embedding_pair(add):
+    """add == add(embedding(W, idx), embedding(P, pos)) with pos 1-D along idx's last dimension
+    (GPT-2's `wte(idx) + wpe(pos)`), each embedding read only by the add, tables of one dtype and
+    the sum of embedding(W, idx)'s shape -> (tok, pos) embedding nodes, else None."""
+    pair = _bin(add, aten.add.Tensor)
+    if pair is None or not all(_call(e, aten.embedding.default) and _only_user(e) is add for e in pair):
+        return None
+    vals = [(_val(e.args[0]), _val(e.args[1])) for e in pair]
+    if _val(add) is None or any(w is None or i is None for w, i in vals) or vals[0][0].dtype != vals[1][0].dtype:
+        return None
+    for tok, pos in ((0, 1), (1, 0)):
+        (w, idx), (p, ps) = vals[tok], vals[pos]
+        if ps.dim() == 1 and idx.dim() >= 1 and idx.shape[-1] == ps.shape[0] \
+                and tuple(_val(add).shape) == tuple(idx.shape) + (w.shape[1],):
+            return pair[tok], pair[pos]
+    return None
+
+
+def _tied_lm_gradient(bwd):
+    """bwd == embedding_dense_backward(...) read only by add(X, bwd) where X is, through view ops
+    only, the fresh row-major [V, C] output of a plain gemm.mm (the tied LM-head weight gradient)
+    and the add is the only reader of X's memory -> (add, X), else None."""
+    from . import gemm
+    add = _only_user(bwd)
+    x = _other(_bin(add, aten.add.Tensor), bwd)
+    root = x
+    while _call(root, *_VIEW_ONLY):
+        root = root.args[0]
+    if not _call(root, gemm.mm) or root.kwargs.get("_side") or _memory_readers(x) != [add]:
+        return None
+    xv, bv, av = _val(x), _val(bwd), _val(add)
+    if xv is None or bv is None or av is None or xv.dim() != 2 or xv.stride(1) != 1 \
+            or tuple(xv.shape) != tuple(bv.shape) or tuple(av.shape) != tuple(xv.shape) \
+            or not xv.dtype == bv.dtype == av.dtype:
+        return None
+    return add, x
+
+
+def fuse_embedding(gm):
+    """Token and position embeddings on edb_embed.cu (embed.py):
+        add(embedding(W, idx), embedding(P, pos))      ==>  embedding_fwd(W, idx, P, pos)
+        embedding(W, idx)                              ==>  embedding_fwd(W, idx)
+        add(X, embedding_dense_backward(dy, idx, V, pad, False))
+                                                       ==>  embedding_bwd_acc_(X, dy, idx, pad)
+        embedding_dense_backward(dy, idx, V, pad, False) ==> embedding_bwd(dy, idx, V, pad)
+    The in-place form applies to the tied LM-head gradient (see _tied_lm_gradient): the embedding
+    gradient is added into that buffer, touching only the rows the tokens index, instead of a dense
+    V x C gradient and a V x C add.  Run behind the gemm.mm retargeting of dispatch_compute.
+    scale_grad_by_freq=True is left alone.  -> (forward, backward) nodes rewritten."""
+    from . import embed
+    graph = gm.graph
+    n_fwd = n_bwd = 0
+    for nd in [nd for nd in graph.nodes if _call(nd, aten.add.Tensor)]:
+        m = _embedding_pair(nd)
+        if m is not None:
+            tok, pos = m
+            with graph.inserting_before(nd):
+                new = graph.call_function(embed.embedding_fwd, (*tok.args[:2], *pos.args[:2]))
+            new.meta = dict(nd.meta)
+            nd.replace_all_uses_with(new)
+            _erase_dead(graph, [nd, tok, pos])
+            n_fwd += 1
+    for nd in list(graph.nodes):
+        if _call(nd, aten.embedding.default):
+            nd.target, nd.args, nd.kwargs = embed.embedding_fwd, tuple(nd.args[:2]), {}
+            n_fwd += 1
+        elif _call(nd, aten.embedding_dense_backward.default) and len(nd.args) == 5 \
+                and not nd.kwargs and nd.args[4] is False:
+            dy, idx, V, pad, _ = nd.args
+            tied = _tied_lm_gradient(nd)
+            if tied is not None:
+                add, x = tied
+                with graph.inserting_before(add):
+                    new = graph.call_function(embed.embedding_bwd_acc_, (x, dy, idx, pad))
+                new.meta = dict(add.meta)
+                add.replace_all_uses_with(new)
+                _erase_dead(graph, [add, nd])
+            else:
+                nd.target, nd.args = embed.embedding_bwd, (dy, idx, V, pad)
+            n_bwd += 1
+    if n_fwd or n_bwd:
+        graph.lint()
+        gm.recompile()
+    return n_fwd, n_bwd
+
+
 def parallel_wgrad_gemms(gm):
     """Opt-in (`EDB_GEMM_SIDE=1`): GEMMs whose result is first *computed on* much later (weight
     gradients: read by the optimizer) are launched on a second compute stream and joined right in
@@ -1972,8 +2058,9 @@ def _reshape_views_of(node):
 def dispatch_compute(gm, counts=None):
     """Route bf16 `aten.mm` / `aten.addmm` nodes to the wgmma GEMM (sharded-op kernel dispatch).
     `counts` (a dict), when given, receives the (forward, backward) counts of the RMSNorm, SwiGLU and
-    RoPE rewrites as "rms_norm", "swiglu" and "rope", and the (norm, scale) counts of the gradient
-    clipping rewrite as "clip"."""
+    RoPE rewrites as "rms_norm", "swiglu" and "rope", the (norm, scale) counts of the gradient
+    clipping rewrite as "clip", and the (forward, backward) counts of the embedding rewrite as
+    "embed"."""
     from . import gemm, norm
     native_ln = os.environ.get("EDB_NATIVE_LN", "1") == "1"
     counts = {} if counts is None else counts
@@ -2017,6 +2104,9 @@ def dispatch_compute(gm, counts=None):
                 node.kwargs = {"_pf": node.meta["edb_pf"]}
             n += 1
     gm.recompile()
+    # behind the gemm.mm retargeting: the tied embedding gradient folds into the LM-head GEMM's output
+    counts["embed"] = fuse_embedding(gm) if os.environ.get("EDB_NATIVE_EMBED", "1") == "1" else (0, 0)
+    n += sum(counts["embed"])
     if os.environ.get("EDB_GEMM_SIDE", "0") == "1":
         n += parallel_wgrad_gemms(gm)
     if os.environ.get("EDB_FUSE_EPILOGUE", "1") == "1":

@@ -372,6 +372,28 @@ int edb_rope(void* y, const void* x, const void* cos, const void* sin, int64_t B
              int64_t T, int64_t half, const int64_t* x_strides, const int64_t* y_strides,
              int64_t table_stride_t, int inverse, int dtype, void* stream);
 
+/* Token and position embeddings (edb_embed.cu); tables, y and dy of `dtype` bf16 or f32, ids of
+ * `idx_dtype` EDB_I32 or EDB_I64.  Ids outside the table are never dereferenced: they read zeros
+ * in the forward and add nothing in the backward (validating them is the caller's contract; no
+ * host synchronisation).  16-byte vectors when C, the row strides and every pointer allow it.
+ * edb_embedding_fwd: y [rows, C] = weight[idx] ([V, C] table), plus, when pos_weight is given,
+ *   pos_weight[pos[r % T]] ([Vp, C] table, pos [T], rows a multiple of T), the fp32 sum rounded
+ *   once: bit-identical to aten.embedding (+ aten.add).  Tables and y contiguous.
+ * edb_embedding_bwd: g[v] = T(sum of dy[r] over the rows r with idx[r] == v), summed in fp32 in
+ *   increasing r (deterministic, no float atomics); dy rows `ld_dy` elements apart.
+ *   accumulate = 0: out [V, C] (rows ld_out apart) gets every row, zeros where nothing was indexed
+ *   and for padding_idx: aten.embedding_dense_backward (scale_grad_by_freq = false).
+ *   accumulate = 1: out[v] = T(float(out[v]) + float(g[v])) in place for the indexed rows other
+ *   than padding_idx; no other row of out is read or written.
+ *   `workspace`: edb_embedding_bwd_workspace(rows, V) bytes. */
+int edb_embedding_fwd(void* y, const void* weight, const void* idx, const void* pos_weight,
+                      const void* pos, int64_t rows, int64_t C, int64_t V, int64_t Vp, int64_t T,
+                      int idx_dtype, int dtype, void* stream);
+int edb_embedding_bwd(void* out, int64_t ld_out, const void* dy, int64_t ld_dy, const void* idx,
+                      void* workspace, int64_t rows, int64_t C, int64_t V, int64_t padding_idx,
+                      int accumulate, int idx_dtype, int dtype, void* stream);
+int edb_embedding_bwd_workspace(int64_t rows, int64_t V, size_t* bytes_out);
+
 /* Column sums out[c] = sum_r x[r, c] of a [rows, cols] matrix with row stride `ld` (elements):
  * the bias gradients `aten.sum.dim_IntList(dy, [0], True)` of the sharded graph.  bf16 or f32, fp32
  * accumulation in a fixed order (deterministic).  `workspace`: edb_colsum_workspace(cols) bytes. */
