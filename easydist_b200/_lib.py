@@ -115,6 +115,12 @@ SIGNATURES = {
                          _I64P, _I64P, c_int64, c_int, c_int, c_void_p]),
     "edb_swiglu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
                                c_void_p]),
+    "edb_attn_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
+                             c_int64, c_int64, _I64P, c_float, c_int, c_void_p]),
+    "edb_attn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                             c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, _I64P,
+                             c_float, c_int, c_void_p]),
+    "edb_attn_bwd_workspace": (c_int, [c_int64, c_int64, c_int64, POINTER(c_size_t)]),
     "edb_embedding_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
                                   c_int64, c_int64, c_int64, c_int, c_int, c_void_p]),
     "edb_embedding_bwd": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int64,

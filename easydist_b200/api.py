@@ -181,6 +181,7 @@ def _finish(gm, params, buffers, named_states, args, kwargs, ops, native, io=Non
         info["rms_norm_nodes"] = counts["rms_norm"]
         info["swiglu_nodes"] = counts["swiglu"]
         info["rope_nodes"] = counts["rope"]
+        info["attn_nodes"] = counts["attn"]
         info["clip_nodes"] = counts["clip"]
         info["embed_nodes"] = counts["embed"]
         if ranks is not None and len(ranks) > 1 and (push or info.get("fused")):

@@ -17,8 +17,8 @@ INCLUDE = os.path.join(ROOT, "include")
 LIB_PATH = os.path.join(HERE, "libedb.so")
 BUILD_DIR = os.path.join(HERE, "csrc", "_build")
 
-HEADERS = ["edb_internal.cuh", "edb_vec.cuh"]
-SOURCES = ["edb_runtime.cu", "edb_reshard.cu", "edb_ll.cu", "edb_norm.cu", "edb_rms.cu", "edb_rope.cu", "edb_embed.cu", "edb_loss.cu", "edb_optim.cu", "edb_clip.cu", "edb_gemm.cu"]
+HEADERS = ["edb_internal.cuh", "edb_vec.cuh", "edb_sm90.cuh"]
+SOURCES = ["edb_runtime.cu", "edb_reshard.cu", "edb_ll.cu", "edb_norm.cu", "edb_rms.cu", "edb_rope.cu", "edb_embed.cu", "edb_loss.cu", "edb_optim.cu", "edb_clip.cu", "edb_gemm.cu", "edb_attn.cu"]
 
 ARCH = "arch=compute_90a,code=sm_90a"
 

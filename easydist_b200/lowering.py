@@ -1666,6 +1666,78 @@ def fuse_rope(gm):
     return n_fwd, n_bwd
 
 
+def fuse_attention(gm):
+    """Rewrite fused-attention nodes onto edb_attn.cu (attn.attention_fwd / attn.attention_bwd):
+    ATen's cuDNN op (what SDPA traces to on the H100), its CUDA flash op and the CPU one, each
+    forward together with its backward when that backward reads the forward's own out and
+    logsumexp getitems and the same q, k, v, is_causal and scale, and a forward whose logsumexp
+    nothing reads on its own (no-grad use).  Left on ATen: dropout, an attention mask or bias,
+    return_debug_mask, and a logsumexp read by anything but the matched backward (only the native
+    backward is guaranteed to understand the native logsumexp).  Runs after fuse_rope, whose
+    outputs are the Llama q and k; any strides are accepted.  The rewritten nodes keep the outputs'
+    meta["val"] (the forward's tuple cut to (out, lse)), write their results with those strides
+    and, off the kernel, run the ATen op they replaced.  Returns (forward, backward) counts."""
+    from torch.fx.operator_schemas import normalize_function
+    from . import attn
+    graph = gm.graph
+    n_fwd = n_bwd = 0
+    named = lambda nd: normalize_function(nd.target, tuple(nd.args), dict(nd.kwargs),
+                                          normalize_to_only_use_kwargs=True).kwargs
+    kinds = {op: kind for kind, op in attn.FWD_OPS.items()}
+    for fwd in [nd for nd in graph.nodes if _call(nd, *attn.FWD_OPS.values())]:
+        a, kind = named(fwd), kinds[fwd.target]
+        if a["dropout_p"] != 0 or a.get("attn_mask") is not None or a.get("attn_bias") is not None \
+                or a.get("return_debug_mask"):
+            continue
+        if any(not _call(u, operator.getitem) for u in fwd.users):
+            continue
+        outs = {}
+        for u in fwd.users:
+            outs.setdefault(u.args[1], []).append(u)
+        vals = fwd.meta.get("val")
+        if len(outs.get(0, ())) != 1 or len(outs.get(1, ())) > 1 or not isinstance(vals, (tuple, list)) \
+                or not isinstance(vals[0], torch.Tensor) or not isinstance(vals[1], torch.Tensor) \
+                or tuple(vals[1].shape[:3]) != tuple(vals[0].shape[:3]) \
+                or vals[1].numel() != vals[0].numel() // vals[0].shape[3]:
+            continue
+        q, k, v = a["query"], a["key"], a["value"]
+        out_nd, lse_nd = outs[0][0], (outs.get(1) or [None])[0]
+        rest = [u for i, us in outs.items() if i > 1 for u in us]
+        bwd = _only_user(lse_nd) if lse_nd is not None else None
+        if bwd is not None:
+            if not _call(bwd, attn.BWD_OPS[kind]):
+                continue
+            b = named(bwd)
+            if b["out"] is not out_nd or b["logsumexp"] is not lse_nd or b["query"] is not q \
+                    or b["key"] is not k or b["value"] is not v or b["dropout_p"] != 0 \
+                    or b["is_causal"] != a["is_causal"] or b.get("scale") != a.get("scale") \
+                    or b.get("attn_mask") is not None or b.get("attn_bias") is not None:
+                continue
+            bvals = bwd.meta.get("val")
+            if not isinstance(bvals, (tuple, list)) or not all(isinstance(t, torch.Tensor) for t in bvals):
+                continue
+        elif lse_nd is not None and lse_nd.users:
+            continue
+        if any(set(u.users) - {bwd} for u in rest):
+            continue
+        ov, lv = vals[0], vals[1]
+        fwd.target = attn.attention_fwd
+        fwd.args = (q, k, v, a["is_causal"], a.get("scale"))
+        fwd.kwargs = {"out_stride": list(ov.stride()), "lse_stride": list(lv.stride()), "aten_op": kind}
+        fwd.meta["val"] = (ov, lv)
+        n_fwd += 1
+        if bwd is not None:
+            bwd.target = attn.attention_bwd
+            bwd.args = (b["grad_out"], q, k, v, out_nd, lse_nd, a["is_causal"], a.get("scale"))
+            bwd.kwargs = {"strides": [list(t.stride()) for t in bvals], "aten_op": kind}
+            n_bwd += 1
+        _erase_dead(graph, rest)
+    if n_fwd or n_bwd:
+        graph.lint()
+        gm.recompile()
+    return n_fwd, n_bwd
+
+
 def fuse_optimizer_updates(gm):
     """The re-inplaced update of torch.optim.SGD(momentum, foreach=True),
         _foreach_mul_(bufs, mu); _foreach_add_(bufs, grads[, alpha=a]); _foreach_add_(params, bufs, alpha=-lr)
@@ -2057,8 +2129,8 @@ def _reshape_views_of(node):
 
 def dispatch_compute(gm, counts=None):
     """Route bf16 `aten.mm` / `aten.addmm` nodes to the wgmma GEMM (sharded-op kernel dispatch).
-    `counts` (a dict), when given, receives the (forward, backward) counts of the RMSNorm, SwiGLU and
-    RoPE rewrites as "rms_norm", "swiglu" and "rope", the (norm, scale) counts of the gradient
+    `counts` (a dict), when given, receives the (forward, backward) counts of the RMSNorm, SwiGLU,
+    RoPE and attention rewrites as "rms_norm", "swiglu", "rope" and "attn", the (norm, scale) counts of the gradient
     clipping rewrite as "clip", and the (forward, backward) counts of the embedding rewrite as
     "embed"."""
     from . import gemm, norm
@@ -2073,9 +2145,17 @@ def dispatch_compute(gm, counts=None):
     counts["rms_norm"] = fuse_rms_norm(gm) if os.environ.get("EDB_NATIVE_RMS", "1") == "1" else (0, 0)
     counts["swiglu"] = fuse_swiglu(gm) if os.environ.get("EDB_NATIVE_SWIGLU", "1") == "1" else (0, 0)
     counts["rope"] = fuse_rope(gm) if os.environ.get("EDB_NATIVE_ROPE", "1") == "1" else (0, 0)
+    # behind fuse_rope: the Llama q and k it writes are the attention's inputs.  Only for steps
+    # compiled under torch.use_deterministic_algorithms(True): there ATen's attention backward is
+    # either cuDNN's, whose bits change from run to run even in its deterministic mode, or
+    # FlashAttention-2's deterministic one, 1.5-1.7x slower than edb_attn.cu's; without that request
+    # cuDNN's non-deterministic kernels are faster (DESIGN.md §7)
+    counts["attn"] = fuse_attention(gm) if torch.are_deterministic_algorithms_enabled() \
+        and os.environ.get("EDB_NATIVE_ATTN", "1") == "1" else (0, 0)
     # behind fuse_optimizer_updates: the clip scale folds into the fused SGD node
     counts["clip"] = fuse_grad_clip(gm) if os.environ.get("EDB_NATIVE_CLIP", "1") == "1" else (0, 0)
-    n += sum(counts["rms_norm"]) + sum(counts["swiglu"]) + sum(counts["rope"]) + sum(counts["clip"])
+    n += sum(counts["rms_norm"]) + sum(counts["swiglu"]) + sum(counts["rope"]) + sum(counts["attn"]) \
+        + sum(counts["clip"])
     for node in gm.graph.nodes:
         if node.op != "call_function":
             continue

@@ -372,6 +372,28 @@ int edb_rope(void* y, const void* x, const void* cos, const void* sin, int64_t B
              int64_t T, int64_t half, const int64_t* x_strides, const int64_t* y_strides,
              int64_t table_stride_t, int inverse, int dtype, void* stream);
 
+/* Scaled-dot-product attention (edb_attn.cu) on bf16 q, k, v, out of one shape [B, H, T, hd],
+ * hd 64 or 128, T_q == T_k == T, no dropout or mask; `scale` multiplies q·kᵀ, causal = 1 lets
+ * query i see keys j <= i only.  The last dim of every tensor is contiguous; `strides`
+ * lists the (B, H, T) element strides of each tensor in the order given below.  Pointers must be
+ * 16-byte aligned and the bf16 strides positive multiples of 8 elements (no broadcast views), and
+ * scale positive and finite, else EDB_E_UNSUPPORTED; so is any other hd.  fp32 accumulation and
+ * softmax.
+ * edb_attn_fwd: out = softmax(scale q·kᵀ) v, lse [B, H, T] fp32 = the natural-log row logsumexp of
+ *   scale q·kᵀ.  strides: q, k, v, out, lse (15 values).
+ * edb_attn_bwd: dq, dk, dv of that forward from dout, its out and lse (the lse edb_attn_fwd wrote).
+ *   Deterministic: every element is summed by one thread in a fixed order, no atomics.
+ *   strides: dout, q, k, v, out, dq, dk, dv, lse (27 values).  `workspace`:
+ *   edb_attn_bwd_workspace(B, H, T) bytes, 16-byte aligned. */
+int edb_attn_fwd(void* out, void* lse, const void* q, const void* k, const void* v, int64_t B,
+                 int64_t H, int64_t T, int64_t hd, const int64_t* strides, float scale, int causal,
+                 void* stream);
+int edb_attn_bwd(void* dq, void* dk, void* dv, const void* dout, const void* q, const void* k,
+                 const void* v, const void* out, const void* lse, void* workspace, int64_t B,
+                 int64_t H, int64_t T, int64_t hd, const int64_t* strides, float scale, int causal,
+                 void* stream);
+int edb_attn_bwd_workspace(int64_t B, int64_t H, int64_t T, size_t* bytes);
+
 /* Token and position embeddings (edb_embed.cu); tables, y and dy of `dtype` bf16 or f32, ids of
  * `idx_dtype` EDB_I32 or EDB_I64.  Ids outside the table are never dereferenced: they read zeros
  * in the forward and add nothing in the backward (validating them is the caller's contract; no
